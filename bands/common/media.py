@@ -1,6 +1,6 @@
 """Container I/O for the band scripts (reference: bands/common/io.py VideoWriter :246-305, decord readers).
 
-Codec work is OUT OF SCOPE of the B200 engine (SURVEY.md section 2: CPU codec, lossy).  The reference uses decord +
+Codec work is OUT OF SCOPE of the H100 engine (SURVEY.md section 2: CPU codec, lossy).  The reference uses decord +
 PyAV/libx264, neither of which is installed in this image; OpenCV's capture/writer is, and is used here.  Frames
 cross this boundary as HxWx3 uint8 RGB arrays, exactly what the reference's loops hand to infer().
 """

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""depth_anything band on the B200 engine -- drop-in for the reference's bands/depth_anything.py.
+"""depth_anything band on the H100 engine -- drop-in for the reference's bands/depth_anything.py.
 
 Same plugin surface (SURVEY.md section 8b): module constants/globals, init_model(), infer(img, normalize),
 process_image(args), process_video(args), the CLI flags of bands/depth_anything.py:255-265, the outputs

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""depth_midas band on the B200 engine -- drop-in for the reference's bands/depth_midas.py.
+"""depth_midas band on the H100 engine -- drop-in for the reference's bands/depth_midas.py.
 
 Same plugin surface: BAND / MODELS_VERSIONS, init_model(model_version), infer(img, model_version, normalize),
 process_image(args), process_video(args), the CLI flags of bands/depth_midas.py:182-192, the outputs (depth_midas.mp4|png,

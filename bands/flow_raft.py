@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""flow_raft band on the B200 engine -- drop-in for the reference's bands/flow_raft.py.
+"""flow_raft band on the H100 engine -- drop-in for the reference's bands/flow_raft.py.
 
 Same plugin surface: BAND / ITERATIONS / MODEL constants, init_model(args), infer(args, prev, curr),
 process_video(args), the CLI flags of bands/flow_raft.py:170-189, the outputs (flow_raft.mp4, flow_raft.csv with the

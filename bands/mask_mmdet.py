@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""mask band (mask_mmdet) on the B200 engine -- drop-in for the reference's bands/mask_mmdet.py.
+"""mask band (mask_mmdet) on the H100 engine -- drop-in for the reference's bands/mask_mmdet.py.
 
 Same plugin surface: BAND / CLASSES / CONFIDENCE_THRESHOLD constants, init_model(), process_image(args),
 process_video(args), the CLI flags of bands/mask_mmdet.py:165-174 (-i -o -c --sdf --subpath), the outputs (mask.png|mp4,

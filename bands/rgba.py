@@ -7,7 +7,7 @@ half (depth optionally re-encoded from hue to the heat map, --encoding_depth hue
 Same CLI as reference rgba.py:149-163, same outputs and metadata keys (:166-199).  This band does no inference: it is
 container / pixel-copy work, and the only arithmetic on the path (hue -> heat re-encode of Record3D depth, :62-64) is
 per-pixel numpy as in the reference.  Frames are decoded / encoded with OpenCV (bands/common/media.py): decord, PyAV and
-ffmpeg, which the reference uses (:77,85; common/io.py:246-305), are not in this image, and the B200 has no NVENC block, so
+ffmpeg, which the reference uses (:77,85; common/io.py:246-305), are not in this image, and the engine has no hardware video codec path, so
 "encode on the GPU" is not an option on this part at all (NVDEC exists; see DESIGN.md section 7).
 """
 import argparse

@@ -1,7 +1,7 @@
 """bench.py -- the BASELINE metric: frames/sec at 1080p with depth_anything (ViT-L) AND flow_raft (12 GRU iterations,
-forward + backward flow) computed for every frame of a synthetic clip, at N B200s.
+forward + backward flow) computed for every frame of a synthetic clip, at N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = one chunk of FRAMES_PER_STEP consecutive 1080p frames per GPU pushed through both bands, the way
@@ -16,12 +16,17 @@ the barrier and the max-over-ranks of the timings.
                the bands' video loops) from pinned host frames to pinned host results: every step uploads the chunk to
                each band and downloads the heat-encoded depth frame + (min,max) and the HSV-encoded forward and backward
                flow frames + max displacements of every frame
-  roofline   : gemm_tc_kernel, the tcgen05 implicit-GEMM core that carries >70 % of the step (ViT linears, DPT head
-               convs, RAFT encoder / update-block convs): algorithmic FLOP of all its launches / their CUDA-event time,
-               vs the measured sustained bf16 peak; `groups` breaks it down and adds the attention kernel and the
-               HBM-bound RAFT correlation build (vs the measured copy bandwidth)
+  roofline   : gemm_tc_kernel, the wgmma implicit-GEMM core (ViT linears, DPT head convs, RAFT encoder / update-block
+               convs): algorithmic FLOP of all its launches / their CUDA-event time, vs the H100 SXM data-sheet dense
+               fp16 rate; `groups` breaks it down and adds the attention kernel and the HBM-bound RAFT correlation build
+               (vs the data-sheet HBM3 bandwidth)
   cpu_baseline / --impl reference : the oracle port of the reference's CPU fp32 path (oracle/da.py + oracle/raft.py; the
-               Python reference itself cannot travel to the GPU box) on the host cores, on a bounded sample of frames
+               Python reference itself does not run without its model downloads) on the host cores, on a bounded sample
+               of frames
+  --dump-outputs DIR : after the timed steps, the arrays the last e2e step returned to its caller (depth heat frames and
+               (min, max), forward / backward flow frames and max displacements), as float32 DIR/<name>.npy; the frame
+               arrays as a fixed seeded sample of their elements.  The inputs are the same from run to run, so two builds
+               can be compared output for output.
 """
 import argparse
 import json
@@ -48,16 +53,13 @@ WORKLOAD = ("synthetic 1080p clip, depth_anything ViT-L + flow_raft (12 GRU iter
 
 
 def measured_peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            p = json.load(f)
-        return dict(hbm=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sustained=p["bf16_tflops_sustained"], src="measured")
-    except Exception:
-        return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback")
+    """NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16.  Upper bounds, not reached rates;
+    a card with a lower power limit runs slower clocks under sustained load."""
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -100,8 +102,8 @@ def make_frames(n, h, w, start):
 
 
 def cpu_threads():
-    """torch CPU scales to ~32 threads on the GPU box's host (measured with tools/cpu_threads.py: 8 thr 7.4 s/frame,
-    16: 6.3, 32: 6.0, 64: 7.7, 128: 41 s/frame) -- use the optimum, and say so."""
+    """Threads of the CPU reference leg: torch CPU stops scaling well before the core counts of large hosts, so at most 32
+    (the count is reported with the number)."""
     return min(32, os.cpu_count() or 1)
 
 
@@ -144,23 +146,11 @@ def run_reference(args, rank, world):
                    "raft_scale": RAFT_SCALE, "frames_per_step": 1},
         "cpu_baseline": {"value": fps, "unit": "frames/s", "cores": cores, "kind": "port",
                          "sample": f"{steps} frames of the 1080p clip, each through oracle/da.py (ViT-L + encode) and oracle/raft.py "
-                                   f"(12 iterations, fwd+bwd, + process_flow), torch CPU fp32, {cores} threads (the measured optimum) "
+                                   f"(12 iterations, fwd+bwd, + process_flow), torch CPU fp32, {cores} threads "
                                    f"of {os.cpu_count()} host cores; no warm-up step (one frame costs tens of seconds)"},
         "e2e": {"value": fps, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
     print(json.dumps(out), flush=True)
-
-
-def measured_traffic():
-    """DRAM bytes per launch of the profiled kernels from the committed ncu --set full captures (profiles/)."""
-    for name in ("r02c_traffic.json", "r02_traffic.json", "r01_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                t = json.load(f)
-            return t.get("traffic_bytes_per_launch"), t
-        except Exception:
-            continue
-    return None, None
 
 
 def corr_build_block(device, peaks):
@@ -180,11 +170,9 @@ def corr_build_block(device, peaks):
     check(l.prisma_flowcorr_work(h, work))
     l.prisma_engine_destroy(h)
     gbs = work[1] / (ms.value * 1e-3) / 1e9
-    tr = (measured_traffic()[1] or {}).get("corr_level0", {})
     return {"bound": "hbm", "kernel": "gemm_tc_kernel (RAFT all-pairs correlation pyramid: 2 GEMMs per direction (level 0; levels 1-3 side by side), K = 256 / 512, fp32 output)",
             "achieved": gbs, "peak": peaks["hbm"], "unit": "GB/s", "frac": gbs / peaks["hbm"], "ms_per_build": ms.value,
-            "algorithmic_bytes": work[1], "traffic": tr.get("traffic_bytes_per_launch"), "traffic_detail": tr or None,
-            "peak_source": peaks["src"],
+            "algorithmic_bytes": work[1], "peak_source": peaks["src"],
             "note": "4-level fp32 pyramid written once (levels 1-3 by linearity: GEMMs against pooled features), timed alone, back to back"}
 
 
@@ -261,11 +249,26 @@ def raft_extra_kernels(pairs):
     return (2 * pairs - 1) + 0 + (4 * pairs - 1) + (6 * pairs - 1) - 1
 
 
+DUMP_SAMPLE = 1 << 21  # elements kept of each frame array: 3 arrays x 8 MB of float32
+
+
+def dump_outputs(path, arrays):
+    """float32 DIR/<name>.npy of each output; arrays larger than DUMP_SAMPLE elements as the same seeded sample of flat
+    indices in every run (the shapes are fixed by the workload)."""
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a).reshape(-1)
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            a = a[idx]
+        np.save(os.path.join(path, name + ".npy"), a.astype(np.float32))
+
+
 def run_b200(args, rank, local_rank, world):
     import torch
     from prisma_b200.depth import DepthAnythingEngine, pinned_empty
     from prisma_b200.flow import RaftFlowEngine
-    from prisma_b200.seeded_weights import make_da_weights, make_raft_weights   # the B200 arm never touches oracle/
+    from prisma_b200.seeded_weights import make_da_weights, make_raft_weights   # the CUDA arm never touches oracle/
 
     dist = None
     if world > 1:
@@ -299,9 +302,13 @@ def run_b200(args, rank, local_rank, world):
     out_flow = {"fwd_rgb": pinned_empty((FRAMES_PER_STEP, hs, ws, 3), np.uint8),
                 "bwd_rgb": pinned_empty((FRAMES_PER_STEP, hs, ws, 3), np.uint8)}
 
+    last = {}
+
     def e2e_step(cont):
-        da.infer_clip(clip, pass_frames=BATCH, out_rgb=out_depth_rgb)
+        _, mins, maxs, _ = da.infer_clip(clip, pass_frames=BATCH, out_rgb=out_depth_rgb)
         r = raft.infer_clip(clip, continue_clip=cont, want_flow=False, want_rgb=True, out=out_flow)
+        last.update(depth_rgb=out_depth_rgb, depth_min=mins, depth_max=maxs, flow_fwd_rgb=r["fwd_rgb"],
+                    flow_bwd_rgb=r["bwd_rgb"], flow_max_fwd=r["max_fwd"], flow_max_bwd=r["max_bwd"])
         return r["pairs"]
 
     # ---------------- e2e: public API, H2D + D2H inside the timed region.  The clip continues from step to step (every
@@ -318,6 +325,8 @@ def run_b200(args, rank, local_rank, world):
     torch.cuda.synchronize(local_rank)
     e2e_s = max_over_ranks(time.perf_counter() - t0)
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # ---------------- value: the chunk resident in HBM, CUDA events on each engine's stream (inside the C ABI)
     da.time_resident(H, W, warm, BATCH)
@@ -356,17 +365,17 @@ def run_b200(args, rank, local_rank, world):
                        "raft_scale": RAFT_SCALE, "frames_per_step": FRAMES_PER_STEP, "depth_frames_per_pass": BATCH,
                        "flow_pairs_per_pass": rf_np, "parallelism": f"frame-sharded x{world}",
                        "l2": "working set per step (0.6 GB fp16 ViT-L weights, 3.6 GB correlation pyramids per pair, activations) "
-                             "exceeds the 126 MB L2; no flush needed"},
+                             "exceeds the 50 MB L2; no flush needed"},
             "e2e": {"value": total_frames / e2e_s, "unit": "frames/s",
                     "h2d_bytes_per_step": 2 * FRAMES_PER_STEP * H * W * 3,   # each band uploads the chunk
                     "d2h_bytes_per_step": FRAMES_PER_STEP * (H * W * 3 + 8 + 2 * hs * ws * 3 + 8)},
             "gpu_launches": launches_step * args.steps,
             "clocks": clocks,
             "roofline": {"bound": "tensor",
-                         "kernel": "gemm_tc_kernel (every tcgen05 contraction of the step: ViT-L linears, DPT head convs, RAFT "
+                         "kernel": "gemm_tc_kernel (every wgmma contraction of the step: ViT-L linears, DPT head convs, RAFT "
                                    "encoder / motion / ConvGRU / head convs)",
                          "achieved": gemm_tf, "peak": peaks["tf_sustained"], "unit": "TFLOP/s", "frac": gemm_tf / peaks["tf_sustained"],
-                         "traffic": measured_traffic()[0], "traffic_detail": measured_traffic()[1], "peak_source": peaks["src"],
+                         "peak_source": peaks["src"],
                          "share_of_step": gemm_ms / step_ms_prof if step_ms_prof > 0 else None,
                          "groups": {
                              "da_encoder_linears": {"tflops": tf(da_work["linear_flop"], da_prof["linear"]), "ms_per_pass": da_prof["linear"],
@@ -404,7 +413,7 @@ def run_b200(args, rank, local_rank, world):
             out["cpu_baseline"] = {"value": fps, "unit": "frames/s", "cores": cores, "kind": "port",
                                    "sample": f"1 frame of the 1080p clip through oracle/da.py (ViT-L + encode) and oracle/raft.py (12 "
                                              f"iterations, fwd+bwd, + process_flow), torch CPU fp32, {cores} threads of "
-                                             f"{os.cpu_count()} host cores (the measured optimum), {dt:.1f} s"}
+                                             f"{os.cpu_count()} host cores, {dt:.1f} s"}
         print(json.dumps(out), flush=True)
     da.close()
     raft.close()
@@ -420,6 +429,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary workloads (other bands)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))

@@ -3,7 +3,7 @@
  *   gcc examples/c_abi_minimal.c -Iinclude -Lprisma_b200 -lprisma_b200 -Wl,-rpath,$PWD/prisma_b200 -o /tmp/prisma_c_abi
  *
  * Prints the library version, the transform sizes of every band for a 1080p frame, and shows the error convention:
- * a negative return code plus a thread-local message (here: creating an engine on a machine without a B200).          */
+ * a negative return code plus a thread-local message (here: creating an engine on a machine without an H100).          */
 #include <stdio.h>
 
 #include "prisma_b200.h"

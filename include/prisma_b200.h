@@ -1,4 +1,4 @@
-/* prisma_b200 -- C ABI of the B200-native per-frame inference engine for PRISMA's band pipeline.
+/* prisma_b200 -- C ABI of the H100-native per-frame inference engine for PRISMA's band pipeline.
  *
  * The reference (patriciogonzalezvivo/prisma @ e00192dd) is pure Python and has no FFI; each entry point
  * below replaces the body of one reference function, cited as file:line relative to the reference root.
@@ -156,7 +156,7 @@ int prisma_flow_infer_resident(prisma_engine* e, int h, int w, double scale, int
 long long prisma_flow_read_tap(prisma_engine* e, const char* name, float* out, long long capacity);
 /* out[0] = algorithmic FLOP of one pass, out[1] = kernel launches per pass, out[2] = hs, out[3] = ws               */
 int prisma_flow_work(prisma_engine* e, int h, int w, double scale, int iters, double* out4);
-/* out[0] / out[1] = algorithmic FLOP of the tcgen05 conv GEMMs of the full / the video pass (encoders, update block, heads;
+/* out[0] / out[1] = algorithmic FLOP of the wgmma conv GEMMs of the full / the video pass (encoders, update block, heads;
  * without the correlation build), out[2] / out[3] = FLOP / algorithmic bytes of one correlation-pyramid build (all 2 * pairs_per_pass
  * directions of a pass; bytes = fp32 pyramid written once + fp16 features read once, raft/corr.py:13-27), out[4] / out[5] = kernel
  * steps of the full / video pass, out[6], out[7] = hs, ws                                                              */
@@ -206,9 +206,9 @@ int prisma_mask_work(prisma_engine* e, int h, int w, double* out8);
 int prisma_net_size(const char* band, int w, int h, int* wn, int* hn);
 
 /* ---- kernel-level entry points (parity tests and micro-benchmarks call the kernels through the C ABI) ---- */
-/* D = A[M,K] * W[N,K]^T (+bias) with fp16 operands / fp32 accumulate on the tcgen05 core; A, W, D host fp32.
+/* D = A[M,K] * W[N,K]^T (+bias) with fp16 operands / fp32 accumulate on the wgmma core; A, W, D host fp32.
  * act: 0 none, 1 gelu, 2 relu; -4 = the TMA-store epilogue (no bias, accumulator scaled by 1/16: the RAFT correlation path).
- * force_bn: 0 = auto, else 32/64/128/256, 512 = CTA pairs.  ms_out (may be NULL): kernel time.                               */
+ * force_bn: 0 = auto, else 32/64/128/256 (512 / 384 / 640: the 256- / 128-wide tiles).  ms_out (may be NULL): kernel time.                               */
 int prisma_debug_gemm(int device, const float* A, const float* W, const float* bias, float* D, int M, int N, int K,
                       int act, int force_bn, int iters, float* ms_out);
 /* The same product through the 3xTF32 path of the mask band (kind::tf32 tensor-core MMAs on [hi | lo] splits of both

@@ -7,7 +7,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("PRISMA_B200_LIB") or os.path.join(_HERE, "libprisma_b200.so")  # override: instrumented builds (tools/)
+LIB_PATH = os.environ.get("PRISMA_B200_LIB") or os.path.join(_HERE, "libprisma_b200.so")  # override: an instrumented build
 _lib = None
 
 c_float_p = C.POINTER(C.c_float)

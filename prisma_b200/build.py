@@ -1,9 +1,9 @@
-"""Build libprisma_b200.so in-tree with nvcc for sm_100a (no torch extension machinery, no JIT cache).
+"""Build libprisma_b200.so in-tree with nvcc for sm_90a (no torch extension machinery, no JIT cache).
 
     python -m prisma_b200.build          # or prisma_b200.build.build()
 
 Objects are rebuilt only when a source or header is newer.  The resulting
-prisma_b200/libprisma_b200.so is git-ignored but travels to the GPU box with the gpurun snapshot.
+prisma_b200/libprisma_b200.so is a build product (git-ignored).
 """
 import concurrent.futures
 import glob
@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libprisma_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -33,7 +33,7 @@ def build(verbose=False, force=False):
     hdrs = glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(HERE, "..", "include", "*.h"))
     newest_hdr = max(os.path.getmtime(h) for h in hdrs)
     nvcc = _nvcc()
-    extra = os.environ.get("PRISMA_NVCC_EXTRA", "").split()  # e.g. -DPRISMA_ATTN_PROFILE for the cycle counters
+    extra = os.environ.get("PRISMA_NVCC_EXTRA", "").split()  # extra nvcc flags, e.g. -Xptxas -v
     jobs = []
     objs = []
     for s in srcs:
@@ -52,7 +52,7 @@ def build(verbose=False, force=False):
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, max(1, len(jobs)))) as ex:
         list(ex.map(run, jobs))
     if jobs or not os.path.exists(LIB):
-        run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart", "-ldl"])
+        run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart", "-ldl"])
     return LIB
 
 

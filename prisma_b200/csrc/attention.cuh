@@ -8,7 +8,6 @@ struct AttnArgs {
   int tokens, heads, D, batch;
   __half* out;
   int out_ld;
-  long long* dbg;  // optional cycle counters (debug builds of the harness only)
 };
 struct AttnLaunch {
   CUtensorMap tm;

@@ -50,7 +50,7 @@ int device_sms(int device, int* sms) {
   PRISMA_CUDA_OK(cudaSetDevice(device));
   cudaDeviceProp prop;
   PRISMA_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  PRISMA_CHECK(prop.major == 10, "prisma_b200 kernels are sm_100a only; there is no fallback path");
+  PRISMA_CHECK(prop.major == 9 && prop.minor == 0, "prisma_b200 kernels are sm_90a only; there is no fallback path");
   *sms = prop.multiProcessorCount;
   return 0;
 }
@@ -82,7 +82,7 @@ extern "C" {
 #pragma GCC visibility push(default)
 
 const char* prisma_last_error(void) { return get_last_error(); }
-const char* prisma_version(void) { return "prisma_b200 0.1 (sm_100a)"; }
+const char* prisma_version(void) { return "prisma_b200 0.1 (sm_90a)"; }
 
 int prisma_device_count(void) {
   int n = 0;
@@ -421,15 +421,7 @@ int prisma_debug_attention(int device, const float* qkv, float* out, int T, int 
   PRISMA_CUDA_OK(cudaMemcpy(dq, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
   AttnLaunch a;
   PRISMA_TRY(attention_prepare(&a, dq, dO, 1, T, heads, D));
-  long long* dbg = sc.alloc<long long>(16);
-  if (getenv("PRISMA_ATTN_PROF")) a.args.dbg = dbg;
   PRISMA_TRY(timed(0, iters > 0 ? iters : 1, ms_out, [&]() { return attention_run(a, 0); }));
-  if (a.args.dbg) {
-    long long h[16];
-    PRISMA_CUDA_OK(cudaMemcpy(h, dbg, sizeof(h), cudaMemcpyDeviceToHost));
-    printf("attention cycles (one softmax warp, CTA (1,1)): wait_S %lld  tmem_ld %lld  max(+rescale) %lld  exp %lld  st+arrive %lld  total %lld  tiles %lld\n"
-           "   lazy rescale of O: %lld cycles in %lld tiles\n", h[0], h[1], h[8], h[2], h[5], h[3], h[4], h[6], h[7]);
-  }
   std::vector<__half> ho((size_t)T * D);
   PRISMA_CUDA_OK(cudaMemcpy(ho.data(), dO, ho.size() * 2, cudaMemcpyDeviceToHost));
   for (size_t i = 0; i < ho.size(); ++i) out[i] = __half2float(ho[i]);

@@ -1,5 +1,5 @@
-// prisma_b200 -- common device/host helpers for sm_100a (B200).
-// Hand-written PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA/TMEM).
+// prisma_b200 -- common device/host helpers for sm_90a (H100).
+// Hand-written PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -72,7 +72,7 @@ __device__ __forceinline__ bool elect_one() {
 // ---- programmatic dependent launch ------------------------------------------------------------------
 // Every kernel of a band's pass begins with pdl_prologue(): (1) griddepcontrol.launch_dependents lets the NEXT kernel of the
 // stream / graph be scheduled as soon as every CTA of this one has started -- its CTAs become resident where resources
-// allow, run their own prologue (barrier init, TMEM allocation, descriptor prefetch) and block in (2) griddepcontrol.wait,
+// allow, run their own prologue (barrier init, descriptor prefetch) and block in (2) griddepcontrol.wait,
 // which returns when the PREVIOUS kernel has completed and its writes are visible.  Nothing touches global memory before
 // the wait, so the dependency chain is the stream order, only the ~2-4 us of launch latency and prologue per kernel
 // overlap the predecessor's tail (a RAFT pass is ~330 kernels of 5-40 us).  Both instructions are no-ops for a kernel
@@ -109,23 +109,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug becomes a trap (-> CUDA error on the host), never a hung GPU box.
+// Bounded wait: a protocol bug becomes a trap (-> CUDA error on the host), never a hung GPU.  No printf here: a function
+// call inside a wgmma kernel makes ptxas serialise its wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s
-      printf("prisma: mbarrier timeout block=(%d,%d) thread=%d bar=%p parity=%u\n", blockIdx.x, blockIdx.y,
-             threadIdx.x, (void*)bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s
   }
-}
-
-__device__ __forceinline__ float fmax3(float a, float b, float c) {  // FMNMX3 (sm_100)
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
 }
 
 // ---- TMA ----------------------------------------------------------------------------------------
@@ -148,172 +139,30 @@ __device__ __forceinline__ void tma_store_wait_read() {  // at most N groups of 
 }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- CTA pairs (cta_group::2): cluster rank / sync, TMA and commits that target the pair ------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> CTA 0 of the pair
-// TMA load issued by either CTA of a pair; the transaction bytes are accounted on the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the leader CTA's copy of a barrier (used by both CTAs' epilogue warps)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {  // one full warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B over the CTA pair: M = 256 (128 rows per CTA), B tile split across the two CTAs
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit -> arrive(1) on the barrier at this smem offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
+// ---- warpgroups -------------------------------------------------------------------------------------
+// register re-allocation between the producer and the consumer warpgroups of a warp-specialised kernel
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// ---- tcgen05 / TMEM -----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp as alloc
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16/bf16 inputs, fp32 accumulate; one thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::tf32: fp32 containers in shared memory (the tensor core uses sign, 8 exponent and the top 10 mantissa bits), fp32
-// accumulate; K = 8 per instruction (32 bytes of a 128-byte swizzled row, like K = 16 of fp16)
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same with the A operand read from TMEM (lanes = rows, 32-bit columns = fp16 pairs along K) instead of shared memory
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit all previously issued tcgen05.mma of this thread -> arrive(1) on an mbarrier when they retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// Shared-memory matrix descriptor, 128B-swizzled tiles whose rows are 128 bytes (64 fp16):
-//   K-major  : rows = M/N index, 8-row groups 1024 B apart (SBO); K advances inside the 128 B row.
+// wgmma shared-memory matrix descriptor, 128B-swizzled tiles whose rows are 128 bytes (64 fp16 / 32 fp32):
+//   K-major  : rows = M/N index, 8-row groups 1024 B apart (SBO); K advances inside the 128 B row (+32 B = +2 per K step).
 //   MN-major : rows = K index, 128 B = 64 MN elements; 8-row K groups 1024 B apart (SBO).
-// Fields (cute/arch/mma_sm100_desc.hpp SmemDescriptor): addr>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
-// version=1 [46,48) | layout_type [61,64) (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t sbo_bytes = 1024,
-                                                     uint32_t lbo_bytes = 16) {
+// Fields (PTX ISA, "Matrix Descriptor Format" of wgmma): addr>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
+// base offset [49,52) = 0 (1024-aligned tiles) | layout_type [62,64) (1 = SWIZZLE_128B).
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr, uint32_t sbo_bytes = 1024, uint32_t lbo_bytes = 16) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor, kind::f16: D=f32 (c_format=1 @4), A/B = f16 (0) or bf16 (1) @7/@10,
-// a_major @15, b_major @16 (0 = K-major, 1 = MN-major), N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// kind::tf32 instruction descriptor: a_format = b_format = 2 (TF32), D = f32
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// TMEM -> registers: this warp's 32 lanes (lane = accumulator row), 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: this warp's 32 lanes, 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---- misc math ------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
@@ -347,6 +196,10 @@ int make_tmap_2d_f16(CUtensorMap* out, const void* base, uint64_t cols, uint64_t
 // the same for an fp32 tensor (box_cols must be 32 -> 128-byte inner box): the destination of the TMA-store epilogue
 int make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t pitch_elems,
                      uint32_t box_cols, uint32_t box_rows);
+
+// SM count of the current device (cached per device): the grid size of the grid-stride pointwise kernels is a small multiple
+// of it, so every SM gets the same number of resident blocks.
+int device_sm_count();
 
 // Launch with the programmatic-stream-serialization attribute when PRISMA_PDL=1 (default: a plain launch; see gemm.cu for the
 // measurement that turned it off).

@@ -1,7 +1,7 @@
 // prisma_b200 -- Depth-Anything engine: weights -> kernel layouts, per-resolution launch plan, per-frame run.
 //
 // Replaces DPT_DINOv2.forward (bands/d_anything/dpt.py:155-166) and the pre/post-processing around it in
-// bands/depth_anything.py:100-143,215-221 with the sm_100a kernels of this directory.  Data layout in HBM:
+// bands/depth_anything.py:100-143,215-221 with the sm_90a kernels of this directory.  Data layout in HBM:
 //   * residual stream x            fp32 [T][D]            (T = 1 + ph*pw tokens)
 //   * every GEMM operand           fp16, K contiguous     (LayerNorm output, qkv, attention output, MLP hidden)
 //   * DPT feature maps             fp16 NHWC with a one-pixel zero border, pixels flattened to rows, so a 3x3
@@ -103,7 +103,7 @@ int DepthEngine::init(const std::string& enc, int dev) {
   PRISMA_CUDA_OK(cudaSetDevice(dev));
   cudaDeviceProp prop;
   PRISMA_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  PRISMA_CHECK(prop.major == 10, "prisma_b200 kernels are sm_100a only (found sm_" + std::to_string(prop.major) +
+  PRISMA_CHECK(prop.major == 9 && prop.minor == 0, "prisma_b200 kernels are sm_90a only (found sm_" + std::to_string(prop.major) +
                                      std::to_string(prop.minor) + "); there is no fallback path");
   num_sms = prop.multiProcessorCount;
   PRISMA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));

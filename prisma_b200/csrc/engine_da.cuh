@@ -95,7 +95,7 @@ class DepthEngine {
   bool metric = false;  // --metric indoor|outdoor: ZoeDepth head on the relative model, fixed 392 x 518 network input
   std::vector<float> host_pos, host_cls;  // MiDaS: pos-embed resized on the host per resolution (bilinear)
   __half* ro_cat = nullptr;               // MiDaS: [B*P][2D] readout operand
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   // streamed (double-buffered) clip path

@@ -7,7 +7,7 @@
 //     pairs; InstanceNorm statistics are per image so the outputs are the same) and cnet likewise;
 //   * only the last iteration's up-sampling mask / convex up-sampling is computed (test_mode consumes only that one);
 //   * BatchNorm (eval) of cnet is folded into the conv weights; InstanceNorm of fnet is a two-stage reduction +
-//     normalise kernel between convs; every conv is the tcgen05 shifted-row GEMM on zero-bordered NHWC fp16 maps.
+//     normalise kernel between convs; every conv is the wgmma shifted-row GEMM on zero-bordered NHWC fp16 maps.
 #include "engine_raft.cuh"
 
 #include <math.h>
@@ -17,8 +17,8 @@
 namespace prisma {
 
 struct RMap {  // B NHWC fp16 maps in the shared-border layout: `pad` zero columns after every row, `pad` zero rows after every
-               // image (see GemmEpilogue::lead); a 1/8-resolution 1080p pair is 2 x 104 x 182 = 37 856 rows = 296 row tiles =
-               // exactly two waves of 148 CTAs (the symmetric border made it 305 tiles = 2.06 waves)
+               // image (see GemmEpilogue::lead); a 1/8-resolution 1080p pair is 2 x 104 x 182 = 37 856 rows = 296 row tiles
+               // instead of the 305 of a symmetric border: 3 % fewer rows through every conv of the pass
   __half* p = nullptr;
   int B = 0, H = 0, W = 0, C = 0, pad = 1;
   int Hp() const { return H + pad; }
@@ -62,7 +62,7 @@ int RaftEngine::init(int dev) {
   PRISMA_CUDA_OK(cudaSetDevice(dev));
   cudaDeviceProp prop;
   PRISMA_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  PRISMA_CHECK(prop.major == 10, "prisma_b200 kernels are sm_100a only; there is no fallback path");
+  PRISMA_CHECK(prop.major == 9 && prop.minor == 0, "prisma_b200 kernels are sm_90a only; there is no fallback path");
   num_sms = prop.multiProcessorCount;
   device_mem = prop.totalGlobalMem;
   PRISMA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));

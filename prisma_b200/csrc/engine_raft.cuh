@@ -77,7 +77,7 @@ class RaftEngine {
   int build_encoder(const EncW& e, bool inorm, const __half* stem_cols, RMap* out_map128, int B);
   int run_direct(cudaStream_t s, int which = 1);  // which: 1 = full pass, 2 = video pass reusing the previous frame's features
 
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaGraphExec_t graph_exec = nullptr, graph_cached = nullptr;
   int cur_mask = 3;          // steps carry a mask (Step::group): bit 0 = full pass, bit 1 = video pass

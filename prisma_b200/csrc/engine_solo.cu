@@ -5,7 +5,7 @@
 // models/solov2_r101_fpn_3x_coco.py, SURVEY.md section 8c):
 //   test pipeline (datasets/pipelines/transforms.py Resize/Normalize/Pad)          -> k_solo_preprocess
 //   ResNet-101, style "pytorch", frozen BatchNorm (models/backbones/resnet.py)     -> stem im2col GEMM, max-pool, 33 bottlenecks
-//       = 100 tcgen05 shifted-row GEMMs on zero-bordered NHWC fp16 maps, BN folded into weights / bias, ReLU and the
+//       = 100 wgmma shifted-row GEMMs on zero-bordered NHWC fp16 maps, BN folded into weights / bias, ReLU and the
 //       residual add in the epilogue, stride-2 convs evaluated at stride 1 and sub-sampled by the row map
 //   FPN (models/necks/fpn.py:151-204)                                               -> 1x1 / 3x3 GEMMs, nearest-add, [::2]
 //   MaskFeatModule + SOLOV2Head towers (models/dense_heads/solov2_head.py)          -> GEMM -> dense fp32 -> GroupNorm+ReLU
@@ -64,7 +64,7 @@ int SoloEngine::init(const std::string& vin, int dev) {
   PRISMA_CUDA_OK(cudaSetDevice(dev));
   cudaDeviceProp prop;
   PRISMA_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  PRISMA_CHECK(prop.major == 10, "prisma_b200 kernels are sm_100a only; there is no fallback path");
+  PRISMA_CHECK(prop.major == 9 && prop.minor == 0, "prisma_b200 kernels are sm_90a only; there is no fallback path");
   num_sms = prop.multiProcessorCount;
   PRISMA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   PRISMA_CUDA_OK(cudaEventCreate(&ev0));

@@ -52,7 +52,7 @@ class SoloEngine {
   int layers[4] = {3, 4, 23, 3}, scale_long = 1333, scale_short = 800;
   int num_grids[5] = {40, 36, 24, 16, 12};
   float strides[5] = {8, 8, 16, 32, 32};
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaGraphExec_t graph_exec = nullptr;

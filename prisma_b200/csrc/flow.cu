@@ -334,7 +334,7 @@ int FlowCorr::init(int dev, int batch, int h8, int w8, int n_frames, const int* 
   PRISMA_CUDA_OK(cudaSetDevice(dev));
   cudaDeviceProp prop;
   PRISMA_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  PRISMA_CHECK(prop.major == 10, "prisma_b200 kernels are sm_100a only; there is no fallback path");
+  PRISMA_CHECK(prop.major == 9 && prop.minor == 0, "prisma_b200 kernels are sm_90a only; there is no fallback path");
   num_sms = prop.multiProcessorCount;
   PRISMA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   rows_pad = round_up(P, 256);

@@ -1,4 +1,4 @@
-// prisma_b200 -- RAFT band, HBM-bound part: pre-process (K11), all-pairs correlation pyramid (K13+K14, on the tcgen05
+// prisma_b200 -- RAFT band, HBM-bound part: pre-process (K11), all-pairs correlation pyramid (K13+K14, on the wgmma
 // GEMM core), correlation lookup (K15) and HSV flow encode (K20).  See flow.cu.
 #pragma once
 #include <vector>
@@ -36,7 +36,7 @@ class FlowCorr {
   int time_build(int iters, float* ms);
   int read_level(int level, int b, int row0, int nrows, float* out);
 
-  int device = 0, B = 0, H8 = 0, W8 = 0, P = 0, C = 256, num_sms = 148;
+  int device = 0, B = 0, H8 = 0, W8 = 0, P = 0, C = 256, num_sms = 132;
   int lh[4], lw[4], ln[4], lpitch[4];  // level sizes, element counts, row pitch (multiple of 4) of the fp32 volumes
   int NF = 0;                          // frames held
   int f1[8] = {0}, f2[8] = {0};        // frame of image1 / image2 per direction

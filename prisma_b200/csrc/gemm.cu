@@ -1,6 +1,7 @@
-// prisma_b200 -- host side of the tcgen05 shifted-row GEMM: TMA descriptor encode, tile-shape choice, launch.
+// prisma_b200 -- host side of the wgmma shifted-row GEMM: TMA descriptor encode, tile-shape choice, launch.
 #include "gemm_tc.cuh"
 
+#include <atomic>
 #include <mutex>
 
 #include <nvtx3/nvToolsExt.h>
@@ -10,13 +11,24 @@ namespace prisma {
 NvtxRange::NvtxRange(const char* name) { nvtxRangePushA(name); }
 NvtxRange::~NvtxRange() { nvtxRangePop(); }
 
-// Programmatic dependent launch is OFF unless PRISMA_PDL=1.  Measured on B200 (bench.py, 1080p depth + flow): 86.3 frames/s
-// with it, 88.7 without -- the early-resident CTAs of the next kernel take issue slots from the running one and the ~330
-// kernels of a RAFT pass are already back to back inside a CUDA graph -- and tests/test_raft_gpu.py saw a wrong max
-// displacement under it (an ordering it must not change).  Kept only as an experiment switch.
+// Programmatic dependent launch is OFF unless PRISMA_PDL=1: the ~330 kernels of a RAFT pass are already back to back inside
+// a CUDA graph, and tests/test_raft_gpu.py has seen a wrong max displacement under it (an ordering it must not change).
+// Kept only as an experiment switch.
 bool pdl_enabled() {
   static const bool on = [] { const char* e = getenv("PRISMA_PDL"); return e && e[0] == '1'; }();
   return on;
+}
+
+int device_sm_count() {
+  static std::atomic<int> cache[64] = {};  // engines on several threads (mask lanes) query it concurrently
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
+    cache[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
 }
 
 static thread_local std::string g_last_error;
@@ -93,12 +105,11 @@ static int make_tmap_2d_f16_store(CUtensorMap* out, const void* base, uint64_t c
   return 0;
 }
 
-// Tile-N choice: minimise waves x per-tile time.  Per-tile costs are MEASURED on B200 (8192^3 sweep, relative units
-// per 64-wide K block): the 128x256 tile runs at 1351 TF/s, 128x128 at 919 TF/s (L2->SM operand traffic per MMA is
-// 1.5x higher), narrower tiles are smem-read bound; plus a per-tile constant for the drain / epilogue hand-off.
+// Tile-N choice: minimise waves x per-tile time.  The per-tile cost is taken proportional to the operand bytes a tile
+// streams per K block ((128 + BN) rows of 128 B) plus the accumulator drain (BN), a model, not a measurement: wide
+// tiles move fewer operand bytes per FLOP, narrow ones waste less on padding and fill the last wave better.
 int gemm_pick_bn(int M, int N, int num_sms) {
   const int cands[4] = {256, 128, 64, 32};
-  const double tile_cost[4] = {128.0, 94.0, 62.0, 45.0};
   int best = 128;
   double best_cost = 1e30;
   const int tiles_m = ceil_div(M, GEMM_BM);
@@ -107,7 +118,7 @@ int gemm_pick_bn(int M, int N, int num_sms) {
     if (bn > 32 && bn >= 2 * round_up(N, 32)) continue;  // mostly padding
     const int tiles = tiles_m * ceil_div(N, bn);
     const int waves = ceil_div(tiles, num_sms);
-    const double cost = waves * (tile_cost[i] + 6.0);
+    const double cost = waves * (double)(GEMM_BM + 2 * bn);
     if (cost < best_cost) { best_cost = cost; best = bn; }
   }
   return best;
@@ -130,14 +141,13 @@ int gemm_prepare_tf32x3(GemmLaunch* out, const float* A_split, long long a_rows,
   int off[GEMM_MAX_TAPS], acol[GEMM_MAX_TAPS];
   for (int t = 0; t < taps; ++t)
     for (int p = 0; p < 3; ++p) { off[t * 3 + p] = tap_off[t]; acol[t * 3 + p] = p == 1 ? C_half : 0; }
-  // external accumulation (GemmArgs::acc_group): 128-wide tiles at most (the running sums are 64 registers per thread), no
-  // narrow tail tiles.  PRISMA_TF32_ACC_GROUP=0 keeps the whole K inside one TMEM chain (the biased, cheaper variant).
+  // external accumulation (GemmArgs::acc_group): 128-wide tiles at most (the running sums are 64 registers per thread).
+  // PRISMA_TF32_ACC_GROUP=0 keeps the whole K inside one wgmma chain (the biased, cheaper variant).
   static const int acc_group = [] { const char* e = getenv("PRISMA_TF32_ACC_GROUP"); return e ? atoi(e) : 4; }();
   if (acc_group > 0 && force_bn == 0) force_bn = N > 64 ? 128 : (N > 32 ? 64 : 32);
   PRISMA_TRY(gemm_prepare_impl(out, A_split, a_rows, C, 2 * C_half, W3, w_rows, M, N, taps * 3, off, acol, ep, num_sms, force_bn, true));
   out->args.acc_group = acc_group > 0 ? acc_group : 1;
   out->xacc = acc_group > 0 && out->bn <= 128;
-  if (out->xacc) { out->args.n_main = ceil_div(M, GEMM_BM) * ceil_div(N, out->bn); out->args.tail_split = 1; out->tmBt = out->tmB; }
   return 0;
 }
 
@@ -147,43 +157,20 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
   PRISMA_CHECK(taps >= 1 && taps <= GEMM_MAX_TAPS, "gemm: bad tap count");
   PRISMA_CHECK(N % 4 == 0, "gemm: N must be a multiple of 4");
   PRISMA_CHECK(M >= 1 && a_cols >= 1, "gemm: empty problem");
-  // force_bn == 512 requests the CTA-pair kernel (256 x 256 tiles); otherwise it is chosen for large problems
-  static const bool pairs_off = [] { const char* e = getenv("PRISMA_GEMM_PAIRS"); return e && e[0] == '0'; }();
+  // force_bn: 32 / 64 / 128 / 256.  512, 384 and 640 name the 256 x 256, 256 x 128 and transposed 128 x 256 tiles of the
+  // sm_100 build (CTA pairs, swapped operands); Hopper has no such instructions, so they request the 256- / 128-wide tiles.
   int bn = force_bn ? force_bn : gemm_pick_bn(M, N, num_sms);
+  if (bn == 512) bn = 256;
+  else if (bn == 384 || bn == 640) bn = 128;
+  GemmEpilogue ep = ep_in;
   // the TMA-store epilogue exists for 128- and 256-wide tiles; a problem the tile choice gives narrower tiles keeps the
   // register epilogue (same results: the TMA path is an optimisation of the same arithmetic)
-  GemmEpilogue ep = ep_in;
   if (ep.tma_store && (bn == 32 || bn == 64) && !tf32) ep.tma_store = false;
-  int cg = 1;
-  static const bool pair128 = [] { const char* e = getenv("PRISMA_GEMM_PAIR128"); return e && e[0] == '1'; }();
-  if (bn == 512) { bn = 256; cg = 2; }
-  else if (bn == 384) { bn = 128; cg = 2; }  // force: 256 x 128 CTA-pair tiles
-  else if (!force_bn && !pairs_off && !tf32 && bn == 256 && M >= 1024 && N >= 256) cg = 2;
-  else if (!force_bn && !pairs_off && !tf32 && pair128 && bn == 128 && M >= 4096 && N >= 128 && !ep.tma_store) cg = 2;
-  PRISMA_CHECK(!(tf32 && cg == 2), "gemm: the tf32 path has no CTA-pair instantiation");
-  // Transposed tiles (GemmCfg SWAP) when one 128-wide tile covers all output columns: an M = 128 instruction costs the tensor
-  // core >= 128 cycles whatever its N, so 128 x 256 (weights x rows) runs at twice the rate of 128 x 128 (rows x weights).
-  // PRISMA_GEMM_SWAP=0 switches it off; force_bn == 640 requests it.
-  static const bool swap_off = [] { const char* e = getenv("PRISMA_GEMM_SWAP"); return e && e[0] == '0'; }();
-  bool swap = false;
-  if (bn == 640) { bn = 128; cg = 1; swap = true; }
-  else if (!force_bn && !swap_off && !tf32 && cg == 1 && bn == 128 && N <= 128 && M >= 4096 && !ep.tma_store && !ep.head_w && !ep.m_dev) swap = true;
-  else {
-    // 64 output columns: the same transposed tile with the upper 64 weight rows zero (they must exist: w_rows >= 128) -- twice
-    // the MMA work of a 128 x 64 tile, but half the instructions, barriers and TMA boxes per output row (RAFT pass 6.73 -> 6.57 ms per pair).  PRISMA_GEMM_SWAP64=0: off.
-    static const bool swap64 = [] { const char* e = getenv("PRISMA_GEMM_SWAP64"); return !(e && e[0] == '0'); }();
-    if (swap64 && !force_bn && !swap_off && !tf32 && cg == 1 && bn == 64 && N > 32 && N <= 64 && w_rows >= 128 && M >= 4096 &&
-        !ep.tma_store && !ep.head_w && !ep.m_dev) { bn = 128; swap = true; }
-  }
-  PRISMA_CHECK(!swap || (N <= 128 && !tf32 && !ep.tma_store && !ep.head_w), "gemm: transposed tiles need N <= 128, fp16 operands, the plain epilogue");
-  out->swap = swap;
   out->tf32 = tf32;
   out->xacc = false;
   out->args.acc_group = 1;
   const int bke = tf32 ? 32 : 64;  // elements per 128-byte K block
   PRISMA_CHECK(bn == 32 || bn == 64 || bn == 128 || bn == 256, "gemm: unsupported BLOCK_N");
-  PRISMA_CHECK(!swap || a_rows >= 1, "gemm: empty operand");
-  out->cg = cg;
   PRISMA_CHECK(w_rows >= round_up(N, bn), "gemm: weight rows must be padded to a multiple of BLOCK_N");
   const int kchunks = ceil_div(a_cols, bke);
   out->bn = bn;
@@ -195,10 +182,6 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
     static const char* r = getenv("PRISMA_GEMM_RASTER");  // "m" / "n": force (experiments)
     out->args.raster_n = r ? (r[0] == 'n') : (M >= N);
   }
-  {
-    static const int dbg = [] { const char* e = getenv("PRISMA_GEMM_DBG"); return e ? atoi(e) : 0; }();
-    out->args.dbg_mode = dbg;
-  }
   for (int t = 0; t < GEMM_MAX_TAPS; ++t) {
     out->args.tap_off[t] = t < taps ? tap_off[t] : 0;
     out->args.tap_acol[t] = (t < taps && tap_acol) ? tap_acol[t] : 0;
@@ -209,46 +192,12 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
     PRISMA_TRY(make_tmap_2d_f32(&out->tmA, A, (uint64_t)a_pitch, (uint64_t)a_rows, (uint64_t)a_pitch, 32, GEMM_BM));
     PRISMA_TRY(make_tmap_2d_f32(&out->tmB, W, (uint64_t)taps * kchunks * 32, (uint64_t)w_rows, (uint64_t)taps * kchunks * 32, 32, bn));
   } else {
-    PRISMA_TRY(make_tmap_2d_f16(&out->tmA, A, (uint64_t)a_cols, (uint64_t)a_rows, (uint64_t)a_pitch, 64, swap ? 256 : GEMM_BM));
+    PRISMA_TRY(make_tmap_2d_f16(&out->tmA, A, (uint64_t)a_cols, (uint64_t)a_rows, (uint64_t)a_pitch, 64, GEMM_BM));
     PRISMA_TRY(make_tmap_2d_f16(&out->tmB, W, (uint64_t)taps * kchunks * 64, (uint64_t)w_rows,
-                                (uint64_t)taps * kchunks * 64, 64, bn / cg));
+                                (uint64_t)taps * kchunks * 64, 64, bn));
   }
-  const int tiles = ceil_div(M, swap ? 256 : GEMM_BM * cg) * ceil_div(N, bn);
-  const int groups = num_sms / cg;
-  out->grid = (tiles < groups ? tiles : groups) * cg;
-  // Tail tiles: when the last wave is partial, cut its tiles into narrower ones so that it costs a fraction of a full
-  // wave (same measured per-tile costs as gemm_pick_bn).  Only when the narrow tiles still fit one wave.
-  out->args.n_main = tiles;
-  out->args.tail_split = 1;
-  out->tmBt = out->tmB;
-  {
-    static const bool tail_off = [] { const char* e = getenv("PRISMA_GEMM_TAIL"); return e && e[0] == '0'; }();
-    const int full = tiles / groups, rem = tiles % groups;
-    auto cost = [](int w) { return w >= 256 ? 134.0 : (w >= 128 ? 100.0 : (w >= 64 ? 68.0 : 51.0)); };
-    if (!tail_off && !force_bn && !swap && full >= 1 && rem > 0) {
-      int best_split = 1;
-      double best = cost(bn);
-      for (int split = 2; split <= 4; split *= 2) {
-        const int bw = bn / split;
-        if (bw < 32 * cg || rem * split > groups) continue;
-        if (ep.tma_store && ep.out_f16 && bw < 64) continue;  // the fp16 TMA-store epilogue writes 64-column boxes
-        if (cost(bw) < best) { best = cost(bw); best_split = split; }
-      }
-      if (best_split > 1) {
-        out->args.n_main = full * groups;
-        out->args.tail_split = best_split;
-        if (tf32) PRISMA_TRY(make_tmap_2d_f32(&out->tmBt, W, (uint64_t)taps * kchunks * 32, (uint64_t)w_rows,
-                                              (uint64_t)taps * kchunks * 32, 32, bn / best_split));
-        else PRISMA_TRY(make_tmap_2d_f16(&out->tmBt, W, (uint64_t)taps * kchunks * 64, (uint64_t)w_rows,
-                                         (uint64_t)taps * kchunks * 64, 64, bn / best_split / cg));
-      }
-    }
-  }
-  if (ep.m_dev) {  // the tile count is decided on the device: no host-side tail cutting
-    out->args.n_main = tiles;
-    out->args.tail_split = 1;
-    out->tmBt = out->tmB;
-  }
+  const int tiles = ceil_div(M, GEMM_BM) * ceil_div(N, bn);
+  out->grid = tiles < num_sms ? tiles : num_sms;
   out->flops = 2.0 * M * (double)N * taps * a_cols;
   // TMA-store epilogue: a plain dense fp32 output (scale only) leaves through swizzled shared-memory boxes and
   // cp.async.bulk.tensor stores instead of per-lane st.global (the store-bound RAFT correlation volume)
@@ -273,36 +222,16 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
   return 0;
 }
 
-template <int BN, int CG, bool TMAST = false, bool TF32 = false, bool XACC = false, bool SWAP = false, int EW = GEMM_EPI_WARPS>
+template <int BN, bool TMAST = false, bool TF32 = false, bool XACC = false>
 static int launch_bn(const GemmLaunch& g, cudaStream_t stream) {
   static bool attr_set = false;  // per-process, per-instantiation
-  using Cfg = GemmCfg<BN, CG, TMAST, SWAP, EW>;
+  using Cfg = GemmCfg<BN, TMAST>;
   if (!attr_set) {
-    PRISMA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, CG, TMAST, TF32, XACC, SWAP, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    PRISMA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, TMAST, TF32, XACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
-  {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(g.grid);
-    cfg.blockDim = dim3(Cfg::THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (CG == 2) {
-      attr[na].id = cudaLaunchAttributeClusterDimension;
-      attr[na].val.clusterDim.x = CG; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-      ++na;
-    }
-    if (pdl_enabled()) {  // the kernel waits (griddepcontrol.wait) after its prologue: safe after any predecessor
-      attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[na].val.programmaticStreamSerializationAllowed = 1;
-      ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    PRISMA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CG, TMAST, TF32, XACC, SWAP, EW>, g.tmA, g.tmB, g.tmBt, g.tmD, g.args));
-  }
+  PRISMA_CUDA_OK(pdl_launch(gemm_tc_kernel<BN, TMAST, TF32, XACC>, dim3(g.grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream,
+                            g.tmA, g.tmB, g.tmD, g.args));
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -310,73 +239,34 @@ static int launch_bn(const GemmLaunch& g, cudaStream_t stream) {
 int gemm_run(const GemmLaunch& g, cudaStream_t stream) {
   if (g.tf32 && g.xacc) {
     switch (g.bn) {
-      case 128: return launch_bn<128, 1, false, true, true>(g, stream);
-      case 64: return launch_bn<64, 1, false, true, true>(g, stream);
-      case 32: return launch_bn<32, 1, false, true, true>(g, stream);
+      case 128: return launch_bn<128, false, true, true>(g, stream);
+      case 64: return launch_bn<64, false, true, true>(g, stream);
+      case 32: return launch_bn<32, false, true, true>(g, stream);
     }
     set_last_error("gemm_run: external accumulation needs BLOCK_N <= 128");
     return -1;
   }
   if (g.tf32) {
     switch (g.bn) {
-      case 256: return launch_bn<256, 1, false, true>(g, stream);
-      case 128: return launch_bn<128, 1, false, true>(g, stream);
-      case 64: return launch_bn<64, 1, false, true>(g, stream);
-      case 32: return launch_bn<32, 1, false, true>(g, stream);
+      case 256: return launch_bn<256, false, true>(g, stream);
+      case 128: return launch_bn<128, false, true>(g, stream);
+      case 64: return launch_bn<64, false, true>(g, stream);
+      case 32: return launch_bn<32, false, true>(g, stream);
     }
     set_last_error("gemm_run: unsupported BLOCK_N (tf32)");
     return -1;
   }
-  // 16 epilogue warps for the plain fp16 kernels (GemmCfg EW).
-  // Measured (same box, whole bench step): 16 warps everywhere: RAFT convs 4.53 -> 4.34 ms per pair but DA linears 16.7 ->
-  // 17.4 ms per pass and head convs 7.05 -> 7.38 (the 256-wide tiles lose an operand stage and spill 270 bytes per thread at the
-  // 96 registers ptxas then allocates).  Default: 16 for the transposed / narrow tiles, 8 for the 256-wide ones;
-  // PRISMA_GEMM_EW=8 / 16 forces one value everywhere.
-  static const int ew_env = [] { const char* e = getenv("PRISMA_GEMM_EW"); return e ? atoi(e) : 0; }();
-  static const int ew_narrow = [] { const char* e = getenv("PRISMA_GEMM_EW_NARROW"); return e ? atoi(e) : 16; }();  // 8 / 12 / 16
-  static const int ew_wide = [] { const char* e = getenv("PRISMA_GEMM_EW_WIDE"); return e ? atoi(e) : 8; }();
-  const int ew = ew_env ? ew_env : ((g.swap || (g.cg == 1 && g.bn <= 128)) ? ew_narrow : ew_wide);
-  if (ew == 16 && !g.tma_store) {
-    if (g.swap) return launch_bn<128, 1, false, false, false, true, 16>(g, stream);
-    if (g.cg == 2 && g.bn == 256) return launch_bn<256, 2, false, false, false, false, 16>(g, stream);
-    if (g.cg == 1) {
-      switch (g.bn) {
-        case 256: return launch_bn<256, 1, false, false, false, false, 16>(g, stream);
-        case 128: return launch_bn<128, 1, false, false, false, false, 16>(g, stream);
-        case 64: return launch_bn<64, 1, false, false, false, false, 16>(g, stream);
-      }
-    }
-  }
-  if (ew == 12 && !g.tma_store) {
-    if (g.swap) return launch_bn<128, 1, false, false, false, true, 12>(g, stream);
-    if (g.cg == 2 && g.bn == 256) return launch_bn<256, 2, false, false, false, false, 12>(g, stream);
-    if (g.cg == 1) {
-      switch (g.bn) {
-        case 256: return launch_bn<256, 1, false, false, false, false, 12>(g, stream);
-        case 128: return launch_bn<128, 1, false, false, false, false, 12>(g, stream);
-        case 64: return launch_bn<64, 1, false, false, false, false, 12>(g, stream);
-      }
-    }
-  }
-  if (g.swap) return launch_bn<128, 1, false, false, false, true>(g, stream);
   if (g.tma_store) {
-    if (g.cg == 2 && g.bn == 256) return launch_bn<256, 2, true>(g, stream);
-    if (g.cg == 1 && g.bn == 256) return launch_bn<256, 1, true>(g, stream);
-    if (g.cg == 1 && g.bn == 128) return launch_bn<128, 1, true>(g, stream);
+    if (g.bn == 256) return launch_bn<256, true>(g, stream);
+    if (g.bn == 128) return launch_bn<128, true>(g, stream);
     set_last_error("gemm_run: no TMA-store instantiation for this tile shape");
     return -1;
   }
-  if (g.cg == 2) {
-    if (g.bn == 256) return launch_bn<256, 2>(g, stream);
-    if (g.bn == 128) return launch_bn<128, 2>(g, stream);
-    set_last_error("gemm_run: CTA pairs need BLOCK_N 256 or 128");
-    return -1;
-  }
   switch (g.bn) {
-    case 256: return launch_bn<256, 1>(g, stream);
-    case 128: return launch_bn<128, 1>(g, stream);
-    case 64: return launch_bn<64, 1>(g, stream);
-    case 32: return launch_bn<32, 1>(g, stream);
+    case 256: return launch_bn<256>(g, stream);
+    case 128: return launch_bn<128>(g, stream);
+    case 64: return launch_bn<64>(g, stream);
+    case 32: return launch_bn<32>(g, stream);
   }
   set_last_error("gemm_run: unsupported BLOCK_N");
   return -1;

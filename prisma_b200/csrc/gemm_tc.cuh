@@ -1,4 +1,4 @@
-// prisma_b200 -- the tcgen05 "shifted-row GEMM" core (sm_100a).
+// prisma_b200 -- the wgmma "shifted-row GEMM" core (sm_90a).
 //
 //   D[m, n] = sum_{t < taps} sum_{c < Cin} A[m + tap_off[t], c] * W[n, t * kchunks*64 + c]        (fp16 x fp16 -> fp32)
 //
@@ -8,23 +8,24 @@
 //                             rows.  Border rows are computed and discarded (waste 2/(W+2)); no im2col buffer, no 4-D
 //                             tensor map; TMA zero-fills out-of-range rows (either sign).
 //
-// Kernel anatomy (persistent, warp-specialised, one CTA per SM):
-//   warp 0   : TMA producer  (A 128x64 and W BNx64 fp16 tiles, 128B swizzle, STAGES-deep mbarrier ring)
-//   warp 1   : MMA issuer    (one lane: tcgen05.mma cta_group::1 kind::f16, M=128, N=BN, K=16; fp32 accum in TMEM,
-//                             two accumulator stages so the epilogue of tile i overlaps the mainloop of tile i+1)
-//   warps 2-9: epilogue      (tcgen05.ld 32x32b -> registers -> smem transpose -> bias / GELU / ReLU / LayerScale /
-//                             residuals -> coalesced fp32 and/or fp16 stores with the row mapping of the consumer's
-//                             layout; two warps per TMEM lane quarter take alternate 32-column chunks; every
-//                             global access of a chunk is issued as a batch of 8 independent requests per lane)
+// Kernel anatomy (persistent, warp-specialised, one CTA per SM, 384 threads):
+//   warpgroups 0-1 : consumers  (each: wgmma.mma_async M=64 x N=BN x K=16 over its 64 rows of the 128-row tile, fp32
+//                                accumulators in registers; then the epilogue of those rows)
+//   warpgroup  2   : producer   (one thread: TMA loads of A 128x64 and W BNx64 fp16 tiles, 128B swizzle, STAGES-deep
+//                                mbarrier ring; its registers are handed to the consumers with setmaxnreg)
+// Epilogue: a warp holds 16 accumulator rows; the two warps of a pair (32 consecutive rows) exchange their fragments through
+// their swizzled 32 x 32 fp32 staging buffers, so that each then owns one 32-row x 32-column chunk and applies bias / GELU /
+// ReLU / LayerScale / residuals with coalesced fp32 and/or fp16 stores in the row mapping of the consumer's layout (every
+// global access of a chunk is issued as a batch of 8 independent requests per lane), or stores it with TMA.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace prisma {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_EPI_WARPS = 8;                          // two per TMEM lane quarter (EW template parameter: 8 or 16)
-constexpr int GEMM_THREADS = 64 + 32 * GEMM_EPI_WARPS;      // + TMA producer warp + MMA warp
+constexpr int GEMM_THREADS = 384;                           // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int GEMM_SMEM_MAX = 232448;                       // 227 KB of dynamic shared memory per CTA
 constexpr int GEMM_MAX_TAPS = 49;
 
@@ -87,8 +88,8 @@ struct GemmEpilogue {
   // Row count known only on the device (SOLOv2: the number of candidates of this frame): when set, only the first
   // round_up(*m_dev, 128) rows of the output space are computed (the launch is sized for the capacity M).
   const int* m_dev = nullptr;
-  // dense output (row_map LINEAR; out_f32: scale only; out_f16: scale, bias, GELU / ReLU) stored by TMA: tcgen05.ld ->
-  // registers (row per lane) -> swizzled smem box -> cp.async.bulk.tensor
+  // dense output (row_map LINEAR; out_f32: scale, bias, LayerScale; out_f16: scale, bias, GELU / ReLU) stored by TMA:
+  // accumulator registers -> swizzled smem box -> cp.async.bulk.tensor
   bool tma_store = false;
   // set by gemm_prepare when tma_store is asked for an in-place fp32 residual update (res_f32 == out_f32: the ViT proj / fc2
   // linears, x += gamma (acc + bias)): the staged box leaves through cp.reduce.async.bulk.tensor ... .add.f32 -- the add is
@@ -114,41 +115,22 @@ struct GemmArgs {
   int tap_off[GEMM_MAX_TAPS];
   int tap_acol[GEMM_MAX_TAPS];  // first A column (elements) of each tap's K slab: 0 for plain convs; the 3xTF32 path walks
                                 // [hi | lo] activation halves: (hi, W_hi), (lo, W_hi), (hi, W_lo)
-  int n_main;      // work items [0, n_main) are full BN-wide tiles; the remaining tiles are each cut into `tail_split`
-  int tail_split;  // narrower tiles (BN / tail_split wide) so the last partial wave costs a fraction of a full one; 1 = off
-  int acc_group;  // XACC kernels: K blocks accumulated inside one TMEM chain before the partial sum is added to the running
-                  // fp32 sums held in the epilogue warps' registers (see gemm_prepare_tf32x3)
-  int dbg_mode;  // diagnostics (PRISMA_GEMM_DBG): 1 = prologue + teardown only, 2 = loads + MMAs but the epilogue warps only
-                 // release the accumulators, 3 = loads only (the MMA warp commits without issuing), 4 = taps one row after
-                 // the previous tap skip their A load, 5 = no loads (MMAs on whatever shared memory holds), 6 = 5 + no epilogue
+  int acc_group;  // XACC kernels: K blocks accumulated inside one wgmma chain before the partial sum is added to the running
+                  // fp32 sums with round-to-nearest FADDs (see gemm_prepare_tf32x3)
   int raster_n;  // 1: consecutive tiles walk N first (the CTAs of a wave share few A row panels and all of W: A is read
                  // from HBM once when M >> N); 0: M first
   GemmEpilogue ep;
 };
 
-// SWAP ("swap A/B", BN == 128, CG == 1): the tensor core spends >= 128 cycles on every M = 128 instruction whatever its N
-// (measured, tools/gemm_pace.py: N = 128 tiles reach half the rate of N = 256 ones with no loads and no epilogue), so a
-// GEMM with <= 128 output columns runs transposed: the WEIGHT tile (128 output channels) is the M operand, 256 pixel rows
-// are the N operand of one instruction, the accumulator holds channels in its lanes and pixels in its columns, and the
-// epilogue transposes through its staging buffer (which it does anyway).  Half the instructions, barriers and TMA boxes
-// per FLOP; the operand bytes per FLOP drop by a quarter.
-// EW: epilogue warps (EW / 4 per TMEM lane quarter, taking every (EW / 4)-th 32-column chunk).  The epilogue is latency-bound
-// (ncu on fc1: issue slots 25 % busy, long-scoreboard / wait stalls) and paces the kernel (DESIGN 4.1), so the fp16 kernels can
-// run 16 of them: half the chunks per warp; one operand stage is given up for the staging buffers and the register cap
-// drops: 18 warps put 5 on one scheduler's 16 K registers = 96 per thread (spills 100-280 bytes), 14 warps (EW = 12) keep 128
-// (spills 40-64 bytes).
-template <int BN, int CG = 1, bool TMAST = false, bool SWAP = false, int EW = GEMM_EPI_WARPS>  // CG = CTAs per MMA (cta_group): 2 = a CTA pair computes a 256 x BN tile, each loading half of W
-struct GemmCfg {                                   // TMAST: TMA-store epilogue (double-buffered staging, one operand stage fewer)
-  static constexpr int A_ROWS = SWAP ? 256 : GEMM_BM;   // activation rows per tile and CTA
-  static constexpr int ACC_COLS = SWAP ? 256 : BN;      // TMEM columns of one accumulator stage
-  static constexpr int A_BYTES = A_ROWS * GEMM_BK * 2;
-  static constexpr int B_BYTES = (BN / CG) * GEMM_BK * 2;
+template <int BN, bool TMAST = false>  // TMAST: TMA-store epilogue (double-buffered staging boxes)
+struct GemmCfg {
+  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;  // 128 rows x 128 B (64 fp16, or 32 fp32 on the tf32 path)
+  static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STG_BYTES = EW * 32 * 32 * 4 * (TMAST ? 2 : 1);  // epilogue staging: 32x32 fp32 per warp (x2 buffers)
+  static constexpr int STG_WARP = TMAST ? 8192 : 4096;     // per consumer warp: one (two) 32 x 128 B boxes
+  static constexpr int STG_BYTES = 8 * STG_WARP;
   static constexpr int FIT = (GEMM_SMEM_MAX - STG_BYTES - 1280) / STAGE_BYTES;  // operand stages that fit beside the staging
-  static constexpr int STAGES = FIT > 7 ? 7 : FIT;
-  static constexpr int THREADS = 64 + 32 * EW;
-  static constexpr int TMEM_COLS = (2 * ACC_COLS <= 32) ? 32 : (2 * ACC_COLS <= 64 ? 64 : (2 * ACC_COLS <= 128 ? 128 : (2 * ACC_COLS <= 256 ? 256 : 512)));
+  static constexpr int STAGES = FIT > 8 ? 8 : FIT;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(STAGES >= 3, "too few operand stages");
 };
@@ -156,8 +138,8 @@ struct GemmCfg {                                   // TMAST: TMA-store epilogue 
 #ifdef __CUDACC__
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 // sigmoid / tanh of the fused epilogues: ex2.approx + rcp.approx (relative error ~4e-7, absolute error of tanh ~2e-7) instead
-// of expf + IEEE division / tanhf.  Measured on the RAFT gate conv (37 888 x 256 outputs): the exact versions cost 18 us per
-// launch on top of an 18.8 us kernel; their accuracy is irrelevant next to the fp16 operand rounding (5e-4).
+// of expf + IEEE division / tanhf: far fewer instructions per element, and their accuracy is irrelevant next to the fp16
+// operand rounding (~5e-4).
 __device__ __forceinline__ float sigmoid_f(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 __device__ __forceinline__ float tanh_f(float x) { return 1.0f - __fdividef(2.0f, __expf(2.0f * x) + 1.0f); }
 __device__ __forceinline__ float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }  // nn.Softplus(beta 1, threshold 20)
@@ -299,195 +281,228 @@ __device__ __forceinline__ void epilogue_rows8(const GemmEpilogue& ep, float4 (&
   }
 }
 
-template <int BN, int CG, bool TMAST, bool TF32, bool XACC, bool SWAP = false, int EW = GEMM_EPI_WARPS>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmBt, const __grid_constant__ CUtensorMap tmD,
-               const __grid_constant__ GemmArgs args) {
-  static_assert(!SWAP || (BN == 128 && CG == 1 && !TMAST && !TF32 && !XACC), "SWAP: 128 output channels x 256 pixel rows, fp16, one CTA");
-  static_assert(EW == 8 || ((EW == 12 || EW == 16) && !TMAST && !TF32 && !XACC), "12 / 16 epilogue warps: the plain fp16 kernels only");
-  using Cfg = GemmCfg<BN, CG, TMAST, SWAP, EW>;
-  constexpr int ACC = Cfg::ACC_COLS;
-  constexpr int CSTEP = 32 * (EW / 4);  // column distance between the chunks one warp takes
-  constexpr int STAGES = Cfg::STAGES;
-  constexpr int BKE = TF32 ? 32 : 64;  // elements per 128-byte K block (fp32 containers for kind::tf32, fp16 otherwise)
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) {
-    if (threadIdx.x == 0) printf("prisma: gemm smem base not 1024-aligned\n");
-    __trap();
+// Staging of the accumulator fragment of one warp (16 rows: r0 = 16 * (warp & 1) + lane / 4 and r0 + 8 of its 32-row slab)
+// into the 32 x 128 B swizzled boxes of the warp pair: buffer q (= buf0 + q * stride) receives columns [cb + q * W, + W) of
+// the slab, W = 32 fp32 (raw or scaled for the fp32 TMA store) or 64 fp16 (the fp16 TMA store, bias + activation applied).
+// The 16-byte slot of column group g in row r is g ^ (r & 7): the 128-byte TMA swizzle of a 1024-aligned buffer.
+// Register indices are compile-time (the column block is selected by predicate), so the accumulators stay in registers.
+template <int BN, int MODE>  // MODE 0: raw fp32, 1: fp32 alpha * acc + bias, * gamma, 2: fp16 act(alpha * acc + bias)
+__device__ __forceinline__ void stage_fragment(const float* d, int cb, uint32_t buf0, uint32_t stride, const GemmEpilogue& ep,
+                                               int n0, int N, int warp, int lane) {
+  constexpr int GROUPS = MODE == 2 ? 16 : 8;  // 8-column groups per call
+  const int r0 = (warp & 1) * 16 + (lane >> 2), tq = lane & 3;
+#pragma unroll
+  for (int jg = 0; jg < BN / 8; ++jg) {
+    const int j = jg - cb / 8;
+    if (j < 0 || j >= GROUPS) continue;
+    float x[4] = {d[jg * 4], d[jg * 4 + 1], d[jg * 4 + 2], d[jg * 4 + 3]};  // (r0, c), (r0, c + 1), (r0 + 8, c), (r0 + 8, c + 1)
+    if (MODE != 0) {
+      const int n = n0 + jg * 8 + tq * 2;
+      float2 b = make_float2(0.f, 0.f), g = make_float2(1.f, 1.f);
+      if (n < N) {
+        if (ep.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+        if (MODE == 1 && ep.gamma != nullptr) g = __ldg(reinterpret_cast<const float2*>(ep.gamma + n));
+      }
+      x[0] = fmaf(x[0], ep.alpha, b.x) * g.x; x[1] = fmaf(x[1], ep.alpha, b.y) * g.y;
+      x[2] = fmaf(x[2], ep.alpha, b.x) * g.x; x[3] = fmaf(x[3], ep.alpha, b.y) * g.y;
+      if (MODE == 2 && ep.act == 1) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) x[q] = gelu_erf(x[q]);
+      } else if (MODE == 2 && ep.act == 2) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) x[q] = fmaxf(x[q], 0.f);
+      }
+    }
+    const uint32_t buf = buf0 + (j / (GROUPS / 2)) * stride;
+    const int jj = j % (GROUPS / 2);
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r0 + hr * 8;
+      if (MODE == 2) {
+        const uint32_t a = buf + row * 128 + ((jj ^ (row & 7)) << 4) + tq * 4;
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_half2(x[2 * hr], x[2 * hr + 1])) : "memory");
+      } else {
+        const int cc = jj * 8 + tq * 2;
+        const uint32_t a = buf + row * 128 + ((((cc >> 2)) ^ (row & 7)) << 4) + (cc & 3) * 4;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x[2 * hr]), "f"(x[2 * hr + 1]) : "memory");
+      }
+    }
   }
+}
+
+template <int BN, bool TMAST, bool TF32, bool XACC>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmD, const __grid_constant__ GemmArgs args) {
+  using Cfg = GemmCfg<BN, TMAST>;
+  constexpr int STAGES = Cfg::STAGES;
+  constexpr int BKE = TF32 ? 32 : 64;  // elements per 128-byte K block (fp32 containers for tf32, fp16 otherwise)
+  extern __shared__ __align__(1024) uint8_t smem[];
+  if ((smem_u32(smem) & 1023u) != 0) __trap();  // 128B-swizzle atoms are 1 KB
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
   float* stg_all = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::STG_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
   pdl_launch_dependents();  // the next kernel may be scheduled behind this one (see common.cuh)
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int rank = CG == 2 ? (int)cluster_ctarank() : 0;  // position inside the CTA pair
-  const int group = blockIdx.x / CG, num_groups = gridDim.x / CG;
-  constexpr int TILE_M = SWAP ? 256 : GEMM_BM * CG;
-  const int M_run = args.ep.m_dev ? min(args.M, (*args.ep.m_dev + TILE_M - 1) / TILE_M * TILE_M) : args.M;  // see GemmEpilogue::m_dev
-  const int tiles_m = (M_run + TILE_M - 1) / TILE_M;
+  const int wg = threadIdx.x >> 7;
+  const int M_run = args.ep.m_dev ? min(args.M, (*args.ep.m_dev + GEMM_BM - 1) / GEMM_BM * GEMM_BM) : args.M;  // see GemmEpilogue::m_dev
+  const int tiles_m = (M_run + GEMM_BM - 1) / GEMM_BM;
   const int tiles_n = (args.N + BN - 1) / BN;
   const int num_tiles = tiles_m * tiles_n;
   const int num_kb = args.taps * args.kchunks;
-  // work items: full tiles first, then the tail tiles cut into `split` narrow ones (see GemmArgs::n_main)
-  const int split = args.tail_split, n_main = split > 1 ? args.n_main : num_tiles;
-  const int num_items = n_main + (num_tiles - n_main) * split;
-  const int bw_tail = BN / split;  // width of a tail tile
-  auto item_tile = [&](int item, int* tm, int* tn, int* nsub, int* bw) {
-    int big = item;
-    *nsub = 0; *bw = BN;
-    if (item >= n_main) { const int u = item - n_main; big = n_main + u / split; *nsub = (u % split) * bw_tail; *bw = bw_tail; }
-    *tm = args.raster_n ? big / tiles_n : big % tiles_m;
-    *tn = args.raster_n ? big % tiles_n : big / tiles_m;
+  auto tile_mn = [&](int tile, int* tm, int* tn) {
+    *tm = args.raster_n ? tile / tiles_n : tile % tiles_m;
+    *tn = args.raster_n ? tile % tiles_n : tile / tiles_m;
   };
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], EW * CG); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }  // empty: one arrival per consumer warpgroup
     fence_mbar_init();
   }
-  if (warp == 1) { if (CG == 2) tmem_alloc_pair(tmem_slot, Cfg::TMEM_COLS); else tmem_alloc(tmem_slot, Cfg::TMEM_COLS); }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();  // the peer's barriers must exist before anything targets them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();  // barriers, TMEM and descriptors are set up; from here on the predecessor's results are read
+  __syncthreads();
+  pdl_wait();  // barriers and descriptors are set up; from here on the predecessor's results are read
 
-  if (args.dbg_mode == 1) {
-    // diagnostics: nothing but the prologue and the teardown
-  } else if (warp == 0) {
+  if (wg == 2) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0 && args.dbg_mode != 5 && args.dbg_mode != 6) {  // dbg_mode 5 / 6: no operand loads at all (the MMA warp does not wait)
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 256) {
       int stage = 0; uint32_t phase = 0;
-      for (int tile = group; tile < num_items; tile += num_groups) {
-        int tm, tn, nsub, bw;
-        item_tile(tile, &tm, &tn, &nsub, &bw);
-        const int m0 = tm * TILE_M + rank * GEMM_BM;
-        const int n0 = tn * BN + nsub + rank * (bw / CG);
-        const CUtensorMap* tb = bw == BN ? &tmB : &tmBt;               // the tail map has a (bw / CG)-row box
-        const uint32_t stage_bytes = Cfg::A_BYTES + (bw / CG) * GEMM_BK * 2;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int tm, tn;
+        tile_mn(tile, &tm, &tn);
+        const int m0 = tm * GEMM_BM, n0 = tn * BN;
         int tap = 0, chunk = 0;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
-          // diagnostics (dbg_mode 4): taps that shift the previous tap's rows by exactly one row do not load A at all (the
-          // MMAs read stale tiles; results are garbage) -- the upper bound of what a shared row-halo A tile would save
-          const bool skip_a = args.dbg_mode == 4 && tap > 0 && args.tap_off[tap] == args.tap_off[tap - 1] + 1;
-          if (CG == 2) {
-            // both CTAs' bytes land on the leader's barrier; only the leader arrives (count 1) and posts the total
-            if (rank == 0) mbar_arrive_expect_tx(&full[stage], 2 * (stage_bytes - (skip_a ? Cfg::A_BYTES : 0)));
-            if (!skip_a) tma_load_2d_pair(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], args.tap_acol[tap] + chunk * BKE, m0 + args.tap_off[tap]);
-            tma_load_2d_pair(sB + stage * Cfg::B_BYTES, tb, &full[stage], kb * BKE, n0);
-          } else {
-            mbar_arrive_expect_tx(&full[stage], stage_bytes - (skip_a ? Cfg::A_BYTES : 0));
-            if (!skip_a) tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], args.tap_acol[tap] + chunk * BKE, m0 + args.tap_off[tap]);
-            tma_load_2d(sB + stage * Cfg::B_BYTES, tb, &full[stage], kb * BKE, n0);
-          }
+          mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+          tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], args.tap_acol[tap] + chunk * BKE, m0 + args.tap_off[tap]);
+          tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], kb * BKE, n0);
           if (++chunk == args.kchunks) { chunk = 0; ++tap; }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA of the pair only)
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc_full = SWAP ? make_idesc_f16(128, 256) : (TF32 ? make_idesc_tf32(TILE_M, BN) : make_idesc_f16(TILE_M, BN));
-      const uint32_t idesc_tail = TF32 ? make_idesc_tf32(TILE_M, bw_tail) : make_idesc_f16(TILE_M, bw_tail);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      if (XACC) {
-        // External accumulation: the tensor core adds into its fp32 accumulator by TRUNCATING the aligned addend, a bias
-        // that grows with the length of the chain (measured: 5e-6 of sum |a||w| after ~900 MMAs).  Here a chain is only
-        // `acc_group` K blocks long; every finished partial sum is handed to the epilogue warps (tfull), which add it
-        // to register-resident running sums with round-to-nearest FADDs, and the TMEM stage is reused (tempty).
-        const int G = args.acc_group;
-        int gi = 0;  // partial sums issued so far (TMEM stage = gi & 1)
-        for (int tile = group; tile < num_items; tile += num_groups) {
-          for (int kb = 0; kb < num_kb; ++kb) {
-            const int kg = kb % G;
-            if (kg == 0) { mbar_wait(&tempty[gi & 1], ((gi >> 1) & 1) ^ 1); tc_fence_after(); }
-            const uint32_t tmem_d = tmem_base + (gi & 1) * BN;
-            mbar_wait(&full[stage], phase);
-            tc_fence_after();
-            const uint64_t adesc = make_sdesc_sw128(smem_u32(sA + stage * Cfg::A_BYTES));
-            const uint64_t bdesc = make_sdesc_sw128(smem_u32(sB + stage * Cfg::B_BYTES));
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) {
-              if (TF32) umma_tf32(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc_full, (kg | k) != 0 ? 1u : 0u);
-              else umma_f16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc_full, (kg | k) != 0 ? 1u : 0u);
-            }
-            umma_commit(&empty[stage]);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            if (kg == G - 1 || kb == num_kb - 1) { umma_commit(&tfull[gi & 1]); ++gi; }
-          }
-        }
-      } else
-      for (int tile = group; tile < num_items; tile += num_groups, ++it) {
-        const uint32_t idesc = tile < n_main ? idesc_full : idesc_tail;
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * ACC;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          if (args.dbg_mode != 5 && args.dbg_mode != 6) mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          // SWAP: the weight tile is the M operand, the 256 activation rows the N operand
-          const uint64_t adesc = make_sdesc_sw128(smem_u32(SWAP ? sB + stage * Cfg::B_BYTES : sA + stage * Cfg::A_BYTES));
-          const uint64_t bdesc = make_sdesc_sw128(smem_u32(SWAP ? sA + stage * Cfg::A_BYTES : sB + stage * Cfg::B_BYTES));
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            if (args.dbg_mode == 3) break;
-            // advance 16 fp16 = 32 B along K inside the 128 B swizzled row: +2 in the (addr >> 4) field
-            if (TF32) umma_tf32(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);  // K = 8 fp32 = 32 B
-            else if (CG == 2) umma_f16_pair(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            else umma_f16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          if (CG == 2) umma_commit_pair(&empty[stage]); else umma_commit(&empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (CG == 2) umma_commit_pair(&tfull[as]); else umma_commit(&tfull[as]);
-      }
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue warps (2..9)
-    const int quarter = warp & 3;           // TMEM lane quarter this warp may access
-    const int chunk_par = (warp - 2) >> 2;  // the EW / 4 warps of a quarter take every (EW / 4)-th 32-column chunk
+    // ------------------------------------------------------------------ consumers: MMA + epilogue of 64 rows each
+    setmaxnreg_inc<232>();
+    const int slab = warp >> 1;    // 32-row slab of the tile this warp pair stores (0..3)
+    const int half = warp & 1;     // which 32-column chunk of a 64-column block this warp stores
+    const int pair_bar = 1 + slab;
     const GemmEpilogue& ep = args.ep;
-    const uint32_t stg = smem_u32(stg_all) + (warp - 2) * (TMAST ? 8192 : 4096);
-    uint32_t st_cnt = 0;  // TMAST: chunks stored so far by this warp (staging buffer parity)
+    const uint32_t stg = smem_u32(stg_all) + warp * Cfg::STG_WARP;
+    const uint32_t stg_pair = smem_u32(stg_all) + (warp & ~1) * Cfg::STG_WARP;
+    uint32_t st_cnt = 0;  // TMAST: boxes stored so far by this warp (staging buffer parity)
     const int cg = lane & 7;     // coalesced phase: which 4-column group of the 32-column chunk
     const int rsub = lane >> 3;  // coalesced phase: row offset inside a 4-row step
-    int it = 0;
-    int xgi = 0;  // XACC: partial sums consumed so far
-    for (int tile = group; tile < num_items; tile += num_groups, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      int tm, tn, nsub, bw;
-      item_tile(tile, &tm, &tn, &nsub, &bw);
-      const int m0 = tm * TILE_M + rank * GEMM_BM;
-      const int n0 = tn * BN + nsub;
-      // ---- row mapping of the 32 output rows a chunk covers (lane == row inside the slab): once per tile (the warp's 32
-      // accumulator rows), or -- SWAP, where the accumulator's COLUMNS are the output rows -- once per 32-pixel chunk
+    float acc[BN / 2];
+    float run[XACC ? BN / 2 : 1];
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int tm, tn;
+      tile_mn(tile, &tm, &tn);
+      const int m0 = tm * GEMM_BM, n0 = tn * BN;
+      // ---- mainloop
+      if (XACC) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) run[i] = 0.f;
+      }
+      int prev_stage = -1;  // stage read by the wgmma group still in flight
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint64_t adesc = make_wgmma_desc(smem_u32(sA + stage * Cfg::A_BYTES + wg * 64 * 128));
+        const uint64_t bdesc = make_wgmma_desc(smem_u32(sB + stage * Cfg::B_BYTES));
+        // External accumulation (XACC): the tensor core adds into its fp32 accumulator by TRUNCATING the aligned addend, a
+        // bias that grows with the length of the chain.  Here a chain is only `acc_group` K blocks long; every finished
+        // partial sum is added to register-resident running sums with round-to-nearest FADDs.
+        const bool first = XACC ? (kb % args.acc_group) == 0 : kb == 0;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          // advance 32 B along K inside the 128 B swizzled row: +2 in the (addr >> 4) field
+          if (TF32) Wgmma<BN>::tf32(acc, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0 : 1);
+          else Wgmma<BN>::f16(acc, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0 : 1);
+        }
+        wgmma_commit();
+        // one wgmma group stays in flight while the next stage is waited for: a stage is released when the group that
+        // read it has retired, one K block later; the chain is drained at the end of a tile (and at the end of an XACC
+        // group, whose partial sum is read here)
+        if (XACC && (kb % args.acc_group) == args.acc_group - 1 && kb != num_kb - 1) {
+          wgmma_wait<0>();
+          if ((threadIdx.x & 127) == 0) {
+            if (prev_stage >= 0) mbar_arrive(&empty[prev_stage]);
+            mbar_arrive(&empty[stage]);
+          }
+          prev_stage = -1;
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) run[i] += acc[i];
+        } else {
+          wgmma_wait<1>();
+          if ((threadIdx.x & 127) == 0 && prev_stage >= 0) mbar_arrive(&empty[prev_stage]);
+          prev_stage = stage;
+        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0 && prev_stage >= 0) mbar_arrive(&empty[prev_stage]);
+      if (XACC) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) run[i] += acc[i];
+      }
+      const float* fin = XACC ? run : acc;
+
+      if (TMAST) {
+        // ---- TMA-store path: scaled (+ bias, LayerScale / activation) values straight into the swizzled boxes of the warp
+        // pair, then one cp.async.bulk.tensor store (or reduce-add) per box by lane 0; two boxes per warp so that the store
+        // of one block reads shared memory while the next is being staged
+        const bool f16o = ep.out_f16 != nullptr;
+        const int CB = f16o ? 128 : 64;  // columns of one pair iteration: two boxes of 64 fp16 / 32 fp32 columns
+#pragma unroll 1
+        for (int cb = 0; cb < BN && n0 + cb < args.N; cb += CB) {
+          const uint32_t par = (st_cnt & 1) * 4096;
+          if (st_cnt >= 2) { if (lane == 0) tma_store_wait_read<1>(); __syncwarp(); }
+          named_bar_sync(pair_bar, 64);  // both boxes of this parity are free
+          if (f16o) stage_fragment<BN, 2>(fin, cb, stg_pair + par, Cfg::STG_WARP, ep, n0, args.N, warp, lane);
+          else stage_fragment<BN, 1>(fin, cb, stg_pair + par, Cfg::STG_WARP, ep, n0, args.N, warp, lane);
+          fence_proxy_async_smem();
+          named_bar_sync(pair_bar, 64);
+          if (lane == 0) {
+            const int c = n0 + cb + half * (CB / 2);
+            if (cb + half * (CB / 2) < BN && c < args.N) {
+              if (ep.tma_reduce)
+                asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                                 reinterpret_cast<uint64_t>(&tmD)),
+                             "r"(stg + par), "r"(c), "r"(m0 + slab * 32)
+                             : "memory");
+              else
+                asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                                 reinterpret_cast<uint64_t>(&tmD)),
+                             "r"(stg + par), "r"(c), "r"(m0 + slab * 32)
+                             : "memory");
+            }
+            tma_store_commit();  // an empty group when this warp's box lies beyond N: keeps the parity count of both warps equal
+          }
+          ++st_cnt;
+        }
+        continue;
+      }
+
+      // ---- row mapping of the 32 output rows of this warp pair's slab (lane == row inside the slab)
       int m = 0, valid = 0, drow = 0;
       int ty = 0, tx = 0, img_base = 0;  // token coordinates / image base row for ROW_SHUFFLE
       const int out_ld = ep.out_lead < 0 ? ep.out_pad : ep.out_lead;  // leading border of the destination map
       int dr8[8], ty8[8], tx8[8], ib8[8];
       uint32_t okrows = 0;
-      auto map_rows = [&](const int mbase) {
-        m = mbase + lane;
+      {
+        m = m0 + slab * 32 + lane;
         valid = m < args.M;
         drow = m;
-        ty = 0; tx = 0; img_base = 0;
         if (ep.row_map == ROW_PADDED || ep.row_map == ROW_PAD2TOK) {
           int img = 0, r = m;
           if (ep.img_rows > 0) { img = m / ep.img_rows; r = m - img * ep.img_rows; }
@@ -513,7 +528,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           drow = img_base + (ty + out_ld) * ep.out_wp + tx + out_ld;
         }
         // row mapping of the 8 rows this lane stores in the coalesced phase
-        okrows = 0;
 #pragma unroll
         for (int rr = 0; rr < 8; ++rr) {
           const int row = rr * 4 + rsub;
@@ -525,112 +539,58 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             ib8[rr] = __shfl_sync(0xffffffffu, img_base, row);
           }
         }
-      };
-      if (!SWAP) map_rows(m0 + quarter * 32);
-      // one 32-column chunk of this warp's 32 accumulator rows: r[j] = row `lane`, column c0 + j
-      // bias / LayerScale vectors of a chunk: issued BEFORE the TMEM read is waited for, so the global-load latency hides
-      // behind it (they used to sit between the shared-memory phases, on the critical path of every chunk)
-      auto load_bias_gamma = [&](const int c0, float4& bias4, float4& gamma4) {
-        const int n = SWAP ? n0 + quarter * 32 + cg * 4 : n0 + c0 + cg * 4;
-        bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        gamma4 = make_float4(1.f, 1.f, 1.f, 1.f);
-        if (n < args.N && ep.bias) bias4 = *reinterpret_cast<const float4*>(ep.bias + n);
-        if (n < args.N && ep.gamma) gamma4 = *reinterpret_cast<const float4*>(ep.gamma + n);
-      };
-      auto process_chunk = [&](uint32_t (&r)[32], const int c0, const float4& bias4, const float4& gamma4) {
-        if (TMAST) {
-          // ---- TMA-store path: registers -> swizzled 32 x 128 B box (the XOR of the 16-byte slot with row & 7 IS the
-          // 128-byte TMA swizzle of a 1024-aligned buffer) -> one cp.async.bulk.tensor store by lane 0; two boxes per warp
-          // so the store of chunk i reads shared memory while chunk i + 1 is being staged
-          const uint32_t buf = stg + (st_cnt & 1) * 4096;
-          if (st_cnt >= 2) { if (lane == 0) tma_store_wait_read<1>(); __syncwarp(); }
-          if (ep.bias == nullptr && ep.gamma == nullptr) {
-            // scale only (the correlation volume): keep this path minimal -- it is store-bound and every extra instruction
-            // per element showed (0.75 -> 0.86 ms per pair when the bias / LayerScale code ran unconditionally)
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              sts128(buf + lane * 128 + ((j ^ (lane & 7)) << 4), __uint_as_float(r[4 * j]) * ep.alpha, __uint_as_float(r[4 * j + 1]) * ep.alpha,
-                     __uint_as_float(r[4 * j + 2]) * ep.alpha, __uint_as_float(r[4 * j + 3]) * ep.alpha);
-          } else {
-            const int ncol = n0 + c0;  // column of r[0]; bias / LayerScale: the same addresses in every lane (broadcast loads)
+      }
+#pragma unroll 1
+      for (int cb = 0; cb < BN && n0 + cb < args.N; cb += 64) {
+        named_bar_sync(pair_bar, 64);  // the partner has finished reading its buffer
+        stage_fragment<BN, 0>(fin, cb, stg_pair, Cfg::STG_WARP, ep, n0, args.N, warp, lane);
+        named_bar_sync(pair_bar, 64);
+        const int c0 = cb + half * 32;
+        if (c0 >= BN || n0 + c0 >= args.N) continue;  // warp-uniform
+        if (ep.head_w != nullptr) {
+          // fused DPT output head (N == 32): the lane's own row, all 32 columns
+          if (valid) {
+            float acc_h = ep.head_b;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f), g4 = make_float4(1.f, 1.f, 1.f, 1.f);
-              if (ncol + 4 * j + 4 <= args.N) {
-                if (ep.bias != nullptr) b4 = __ldg(reinterpret_cast<const float4*>(ep.bias + ncol + 4 * j));
-                if (ep.gamma != nullptr) g4 = __ldg(reinterpret_cast<const float4*>(ep.gamma + ncol + 4 * j));
-              }
-              sts128(buf + lane * 128 + ((j ^ (lane & 7)) << 4), fmaf(__uint_as_float(r[4 * j]), ep.alpha, b4.x) * g4.x,
-                     fmaf(__uint_as_float(r[4 * j + 1]), ep.alpha, b4.y) * g4.y, fmaf(__uint_as_float(r[4 * j + 2]), ep.alpha, b4.z) * g4.z,
-                     fmaf(__uint_as_float(r[4 * j + 3]), ep.alpha, b4.w) * g4.w);
-            }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (ep.tma_reduce)
-              asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                               reinterpret_cast<uint64_t>(&tmD)),
-                           "r"(buf), "r"(n0 + c0), "r"(m0 + quarter * 32)
-                           : "memory");
-            else
-              asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                               reinterpret_cast<uint64_t>(&tmD)),
-                           "r"(buf), "r"(n0 + c0), "r"(m0 + quarter * 32)
-                           : "memory");
-            tma_store_commit();
-          }
-          ++st_cnt;
-          return;
-        }
-        if (ep.head_w != nullptr) {
-          if (valid) {
-            float acc = ep.head_b;
+              const float4 q = lds128(stg + lane * 128 + ((j ^ (lane & 7)) << 4));
+              const float r4[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              acc = fmaf(fmaxf(__uint_as_float(r[j]) + __ldg(ep.bias + j), 0.f), __ldg(ep.head_w + j), acc);
+              for (int t = 0; t < 4; ++t) acc_h = fmaf(fmaxf(r4[t] + __ldg(ep.bias + 4 * j + t), 0.f), __ldg(ep.head_w + 4 * j + t), acc_h);
+            }
             int img = 0, rpix = m;
             if (ep.img_rows > 0) { img = m / ep.img_rows; rpix = m - img * ep.img_rows; }
             const int y = rpix / ep.in_w, x = rpix - y * ep.in_w, pd = ep.pad;
             const size_t pix = ((size_t)img * (ep.in_h - 2 * pd) + (y - pd)) * (ep.in_w - 2 * pd) + (x - pd);
-            ep.head_out[pix] = fmaxf(acc, 0.f);
+            ep.head_out[pix] = fmaxf(acc_h, 0.f);
             if (ep.out_f16) {  // also keep the 32 ReLU'd activations (the out_conv hook of the metric head), dense rows
-              uint32_t pk[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                pk[j] = pack_half2(fmaxf(__uint_as_float(r[2 * j]) + __ldg(ep.bias + 2 * j), 0.f),
-                                   fmaxf(__uint_as_float(r[2 * j + 1]) + __ldg(ep.bias + 2 * j + 1), 0.f));
               uint4* dst = reinterpret_cast<uint4*>(ep.out_f16 + pix * ep.out_f16_ld);
 #pragma unroll
-              for (int j = 0; j < 4; ++j) dst[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+              for (int j = 0; j < 4; ++j) {
+                const float4 a = lds128(stg + lane * 128 + (((2 * j) ^ (lane & 7)) << 4));
+                const float4 b = lds128(stg + lane * 128 + (((2 * j + 1) ^ (lane & 7)) << 4));
+                const float* bs = ep.bias + 8 * j;
+                dst[j] = make_uint4(pack_half2(fmaxf(a.x + __ldg(bs), 0.f), fmaxf(a.y + __ldg(bs + 1), 0.f)),
+                                    pack_half2(fmaxf(a.z + __ldg(bs + 2), 0.f), fmaxf(a.w + __ldg(bs + 3), 0.f)),
+                                    pack_half2(fmaxf(b.x + __ldg(bs + 4), 0.f), fmaxf(b.y + __ldg(bs + 5), 0.f)),
+                                    pack_half2(fmaxf(b.z + __ldg(bs + 6), 0.f), fmaxf(b.w + __ldg(bs + 7), 0.f)));
+              }
             }
           }
-          return;
+          continue;
         }
-        // ---- phase 1: row-per-lane registers -> swizzled smem (conflict-free 16 B slots)
-        if (SWAP) {
-          // the lane holds output column (channel) `lane` of the 32 output rows (pixels) c0 .. c0 + 31: element (row j, column
-          // lane) goes to the same swizzled slot the row-per-lane layout uses (32 consecutive words per instruction)
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + j * 128 + ((((lane >> 2) ^ (j & 7))) << 4) + ((lane & 3) << 2)), "r"(r[j]) : "memory");
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            sts128(stg + lane * 128 + ((j ^ (lane & 7)) << 4), __uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                   __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-        }
-        __syncwarp();
-        // ---- phase 2: 8 lanes x 4 columns cover one row's 32 columns; 4 rows per step -> coalesced global access
-        const int n = SWAP ? n0 + quarter * 32 + cg * 4 : n0 + c0 + cg * 4;
+        // ---- coalesced phase: 8 lanes x 4 columns cover one row's 32 columns; 4 rows per step
+        const int n = n0 + c0 + cg * 4;
         const bool ncol_ok = n < args.N;
+        float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f), gamma4 = make_float4(1.f, 1.f, 1.f, 1.f);
+        if (ncol_ok && ep.bias) bias4 = *reinterpret_cast<const float4*>(ep.bias + n);
+        if (ncol_ok && ep.gamma) gamma4 = *reinterpret_cast<const float4*>(ep.gamma + n);
         float4 v[8];
 #pragma unroll
         for (int rr = 0; rr < 8; ++rr) {
           const int row = rr * 4 + rsub;
           v[rr] = lds128(stg + row * 128 + ((cg ^ (row & 7)) << 4));
         }
-        __syncwarp();  // staging may be overwritten by the next chunk from here on
         int col = n;
         if (ep.row_map == ROW_SHUFFLE) {
           const int q = n / ep.shuf_cout;
@@ -640,9 +600,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
           for (int rr = 0; rr < 8; ++rr)
             drs[rr] = ib8[rr] + (ty8[rr] * ep.shuf_s + sdy + out_ld) * ep.out_wp + tx8[rr] * ep.shuf_s + sdx + out_ld;
-          epilogue_rows8<!TF32 && !XACC && !TMAST>(ep, v, drs, ncol_ok ? okrows : 0u, bias4, gamma4, col);
+          epilogue_rows8<!TF32 && !XACC>(ep, v, drs, ncol_ok ? okrows : 0u, bias4, gamma4, col);
         } else {
-          epilogue_rows8<!TF32 && !XACC && !TMAST>(ep, v, dr8, ncol_ok ? okrows : 0u, bias4, gamma4, col);
+          epilogue_rows8<!TF32 && !XACC>(ep, v, dr8, ncol_ok ? okrows : 0u, bias4, gamma4, col);
         }
         if (ep.stat_part != nullptr) {
           float4 sm = make_float4(0.f, 0.f, 0.f, 0.f), sq = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -661,162 +621,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             sq.z += __shfl_xor_sync(0xffffffffu, sq.z, o); sq.w += __shfl_xor_sync(0xffffffffu, sq.w, o);
           }
           if (rsub == 0 && ncol_ok) {
-            const size_t slab = (size_t)(SWAP ? m0 + c0 : m0 + quarter * 32) >> 5;
-            *reinterpret_cast<float4*>(ep.stat_part + (slab * 2) * args.N + n) = sm;
-            *reinterpret_cast<float4*>(ep.stat_part + (slab * 2 + 1) * args.N + n) = sq;
+            const size_t sl = (size_t)(m0 + slab * 32) >> 5;
+            *reinterpret_cast<float4*>(ep.stat_part + (sl * 2) * args.N + n) = sm;
+            *reinterpret_cast<float4*>(ep.stat_part + (sl * 2 + 1) * args.N + n) = sq;
           }
         }
-      
-      };
-      if (XACC) {
-        // running sums of this warp's chunks live in registers; partial sums arrive every `acc_group` K blocks
-        constexpr int NCH = (BN + 63) / 64;
-        float acc[NCH][32];
-#pragma unroll
-        for (int i = 0; i < NCH; ++i)
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[i][j] = 0.f;
-        const int ngroups = (num_kb + args.acc_group - 1) / args.acc_group;
-        for (int g = 0; g < ngroups; ++g, ++xgi) {
-          const int xs = xgi & 1;
-          mbar_wait(&tfull[xs], (xgi >> 1) & 1);
-          tc_fence_after();
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + xs * BN;
-#pragma unroll
-          for (int i = 0; i < NCH; ++i) {
-            const int c0 = chunk_par * 32 + 64 * i;
-            if (c0 < bw && n0 + c0 < args.N) {  // warp-uniform
-              uint32_t r[32];
-              tmem_ld32(taddr + c0, r);
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) acc[i][j] += __uint_as_float(r[j]);
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[xs]);
-        }
-#pragma unroll
-        for (int i = 0; i < NCH; ++i) {
-          const int c0 = chunk_par * 32 + 64 * i;
-          if (c0 < bw && n0 + c0 < args.N) {
-            float4 bias4, gamma4;
-            load_bias_gamma(c0, bias4, gamma4);
-            uint32_t r[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(acc[i][j]);
-            process_chunk(r, c0, bias4, gamma4);
-          }
-        }
-        continue;  // the TMEM stages were released group by group
       }
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * ACC;
-      if (SWAP) {
-        // this warp: output columns n0 + quarter * 32 .. + 31 (TMEM lanes), alternate 32-pixel chunks (TMEM columns)
-#pragma unroll 1
-        for (int c0 = chunk_par * 32; c0 < 256; c0 += CSTEP) {
-          if (m0 + c0 >= args.M || n0 + quarter * 32 >= args.N || args.dbg_mode == 2 || args.dbg_mode == 3 || args.dbg_mode == 6) break;  // warp-uniform
-          uint32_t r[32];
-          tmem_ld32(taddr + c0, r);
-          map_rows(m0 + c0);
-          float4 bias4, gamma4;
-          load_bias_gamma(c0, bias4, gamma4);
-          tmem_ld_wait();
-          process_chunk(r, c0, bias4, gamma4);
-        }
-      } else if (TMAST && ep.out_f16 != nullptr) {
-        // fp16 destination: a warp takes 64-column blocks (two TMEM chunks) so that every bulk store still moves a
-        // 32 x 128-byte box, the same staging layout and swizzle as the fp32 path
-#pragma unroll 1
-        for (int cb = chunk_par * 64; cb < bw; cb += 128) {
-          if (n0 + cb >= args.N || args.dbg_mode == 2 || args.dbg_mode == 3 || args.dbg_mode == 6) break;  // warp-uniform
-          const uint32_t buf = stg + (st_cnt & 1) * 4096;
-          if (st_cnt >= 2) { if (lane == 0) tma_store_wait_read<1>(); __syncwarp(); }
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            const int c0 = cb + hf * 32;
-            if (c0 < bw && n0 + c0 < args.N) {  // warp-uniform; a missing right half lies beyond N and is clipped by the store
-              uint32_t r[32];
-              tmem_ld32(taddr + c0, r);
-              tmem_ld_wait();
-              const int ncol = n0 + c0;  // column of r[0]; every lane holds the same 32 columns of its own row
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                // bias (the same addresses in every lane: one broadcast transaction) + GELU / ReLU in the row-per-lane layout
-                float4 ba = make_float4(0.f, 0.f, 0.f, 0.f), bb = ba;
-                if (ep.bias != nullptr && ncol + 8 * j + 8 <= args.N) {
-                  ba = __ldg(reinterpret_cast<const float4*>(ep.bias + ncol + 8 * j));
-                  bb = __ldg(reinterpret_cast<const float4*>(ep.bias + ncol + 8 * j + 4));
-                }
-                float x[8] = {fmaf(__uint_as_float(r[8 * j]), ep.alpha, ba.x),     fmaf(__uint_as_float(r[8 * j + 1]), ep.alpha, ba.y),
-                              fmaf(__uint_as_float(r[8 * j + 2]), ep.alpha, ba.z), fmaf(__uint_as_float(r[8 * j + 3]), ep.alpha, ba.w),
-                              fmaf(__uint_as_float(r[8 * j + 4]), ep.alpha, bb.x), fmaf(__uint_as_float(r[8 * j + 5]), ep.alpha, bb.y),
-                              fmaf(__uint_as_float(r[8 * j + 6]), ep.alpha, bb.z), fmaf(__uint_as_float(r[8 * j + 7]), ep.alpha, bb.w)};
-                if (ep.act == 1) {
-#pragma unroll
-                  for (int q = 0; q < 8; ++q) x[q] = gelu_erf(x[q]);
-                } else if (ep.act == 2) {
-#pragma unroll
-                  for (int q = 0; q < 8; ++q) x[q] = fmaxf(x[q], 0.f);
-                }
-                const uint32_t h0 = pack_half2(x[0], x[1]), h1 = pack_half2(x[2], x[3]), h2 = pack_half2(x[4], x[5]), h3 = pack_half2(x[6], x[7]);
-                sts128(buf + lane * 128 + (((hf * 4 + j) ^ (lane & 7)) << 4), __uint_as_float(h0), __uint_as_float(h1),
-                       __uint_as_float(h2), __uint_as_float(h3));
-              }
-            }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                             reinterpret_cast<uint64_t>(&tmD)),
-                         "r"(buf), "r"(n0 + cb), "r"(m0 + quarter * 32)
-                         : "memory");
-            tma_store_commit();
-          }
-          ++st_cnt;
-        }
-      } else
-#pragma unroll 1
-      for (int c0 = chunk_par * 32; c0 < bw; c0 += CSTEP) {
-        if (n0 + c0 >= args.N || args.dbg_mode == 2 || args.dbg_mode == 3 || args.dbg_mode == 6) break;  // warp-uniform
-        uint32_t r[32];
-        tmem_ld32(taddr + c0, r);
-        float4 bias4, gamma4;
-        load_bias_gamma(c0, bias4, gamma4);
-        tmem_ld_wait();
-        process_chunk(r, c0, bias4, gamma4);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { if (CG == 2) mbar_arrive_leader(&tempty[as]); else mbar_arrive(&tempty[as]); }
     }
     if (TMAST && lane == 0) tma_store_wait_all();  // shared memory must outlive the last bulk stores
-  }
-  __syncwarp();
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();  // no CTA of a pair may exit while the other can still signal it
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG == 2) tmem_dealloc_pair(tmem_base, Cfg::TMEM_COLS); else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 #endif  // __CUDACC__
 
 // Host-side prepared launch: tensor maps encoded once, replayed every frame (also inside CUDA graphs).
 struct GemmLaunch {
-  CUtensorMap tmA, tmB, tmBt;  // tmBt: W with the narrow box of the tail tiles (== tmB when there is no tail)
-  CUtensorMap tmD;             // dense output, 32 x 32 boxes (TMA-store epilogue only)
+  CUtensorMap tmA, tmB;
+  CUtensorMap tmD;             // dense output, 32-row boxes (TMA-store epilogue only)
   bool tma_store = false;
   bool xacc = false;           // external fp32 accumulation (tf32x3 only): see GemmArgs::acc_group
-  bool tf32 = false;           // kind::tf32 operands (fp32 containers): the 3xTF32 "fp32-class" path of the mask band
-  bool swap = false;           // transposed tiles for N <= 128: 128 output columns x 256 rows per instruction (GemmCfg SWAP)
+  bool tf32 = false;           // tf32 operands (fp32 containers): the 3xTF32 "fp32-class" path of the mask band
   GemmArgs args;
   int bn = 128;
-  int cg = 1;  // 2 = CTA pairs (cta_group::2), 256 x bn tiles
   int grid = 1;
   double flops = 0;  // algorithmic 2*M*N*K (excluding border/padding waste)
 };

@@ -1,4 +1,4 @@
-// prisma_b200 -- RAFT band: the pointwise / gather kernels around the tcgen05 conv core
+// prisma_b200 -- RAFT band: the pointwise / gather kernels around the wgmma conv core
 // (instance norm, im2col of the 7x7 stem, cnet split, GRU gate algebra, coords update, convex up-sampling).
 // Reference: bands/raft/{extractor,update,raft}.py.  All feature maps are NHWC fp16 in the "shared border" layout: `pad`
 // zero columns after every row and `pad` zero rows after every image (gemm_tc.cuh GemmEpilogue::lead), so pixel (y, x) of
@@ -44,7 +44,7 @@ __global__ void k_im2col_stem(const float* __restrict__ x, int B, int H, int W, 
   }
 }
 int raft_im2col_stem(const float* x, int B, int H, int W, __half* out, cudaStream_t s) {
-  PRISMA_CUDA_OK(pdl_launch(k_im2col_stem, dim3(148 * 16), dim3(256), 0, s, x, B, H, W, out));
+  PRISMA_CUDA_OK(pdl_launch(k_im2col_stem, dim3(device_sm_count() * 16), dim3(256), 0, s, x, B, H, W, out));
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -290,7 +290,7 @@ __global__ void k_flow_im2col(const float* __restrict__ coords0, const float* __
   }
 }
 int raft_flow_im2col(const float* coords0, const float* coords1, int B, int H, int W, __half* out, cudaStream_t s) {
-  PRISMA_CUDA_OK(pdl_launch(k_flow_im2col, dim3(148 * 8), dim3(256), 0, s, coords0, coords1, B, H, W, out));
+  PRISMA_CUDA_OK(pdl_launch(k_flow_im2col, dim3(device_sm_count() * 8), dim3(256), 0, s, coords0, coords1, B, H, W, out));
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -43,7 +43,7 @@ __global__ void k_dense_to_split(const float* __restrict__ src, int H, int W, in
   }
 }
 int solo_dense_to_split(const float* src, int H, int W, int Csrc, float* dst, int Cdst, cudaStream_t s) {
-  k_dense_to_split<<<148 * 4, 256, 0, s>>>(src, H, W, Csrc, dst, Cdst);
+  k_dense_to_split<<<device_sm_count() * 4, 256, 0, s>>>(src, H, W, Csrc, dst, Cdst);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -62,7 +62,7 @@ __global__ void k_f16map_to_split(const __half* __restrict__ src, int H, int W, 
   }
 }
 int solo_f16map_to_split(const __half* src, int H, int W, int C, float* dst, int Cdst, cudaStream_t s) {
-  k_f16map_to_split<<<148 * 4, 256, 0, s>>>(src, H, W, C, dst, Cdst);
+  k_f16map_to_split<<<device_sm_count() * 4, 256, 0, s>>>(src, H, W, C, dst, Cdst);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -101,7 +101,7 @@ int gn_stats(const float* x, int HW, int C, int groups, float* part, float* stat
 int groupnorm_relu_split(const float* x, int H, int W, int C, int groups, const float* gamma, const float* beta, float* part,
                          float* stats, float* out_split, float* out_w3, cudaStream_t s) {
   PRISMA_TRY(gn_stats(x, H * W, C, groups, part, stats, s));
-  k_gn_apply_split<<<148 * 4, 256, 0, s>>>(x, H, W, C, stats, gamma, beta, out_split, out_w3);
+  k_gn_apply_split<<<device_sm_count() * 4, 256, 0, s>>>(x, H, W, C, stats, gamma, beta, out_split, out_w3);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -186,7 +186,7 @@ __global__ void k_resize_bilinear_split(const float* __restrict__ src, int Hs, i
 }
 int resize_bilinear_split(const float* src, int Hs, int Ws, int Csrc, int Csrc_pitch, float* dst, int Hd, int Wd, int Cdst, int coord,
                           int accumulate, cudaStream_t s, int dst_frame_w) {
-  k_resize_bilinear_split<<<148 * 4, 256, 0, s>>>(src, Hs, Ws, Csrc, Csrc_pitch, dst, Hd, Wd, Cdst, (float)Hs / (float)Hd,
+  k_resize_bilinear_split<<<device_sm_count() * 4, 256, 0, s>>>(src, Hs, Ws, Csrc, Csrc_pitch, dst, Hd, Wd, Cdst, (float)Hs / (float)Hd,
                                                  (float)Ws / (float)Wd, coord, accumulate, dst_frame_w > 0 ? dst_frame_w : Wd);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -253,7 +253,7 @@ __global__ void k_im2col_stem_split(const float* __restrict__ x, int H, int W, f
   }
 }
 int solo_im2col_stem_split(const float* x, int H, int W, float* out, cudaStream_t s) {
-  k_im2col_stem_split<<<148 * 8, 256, 0, s>>>(x, H, W, out);
+  k_im2col_stem_split<<<device_sm_count() * 8, 256, 0, s>>>(x, H, W, out);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -279,7 +279,7 @@ __global__ void k_maxpool3s2_dense(const float* __restrict__ in, int H, int W, i
   }
 }
 int maxpool3s2_dense(const float* in, int H, int W, int C, float* out, float* out_split, int Ho, int Wo, cudaStream_t s) {
-  k_maxpool3s2_dense<<<148 * 8, 256, 0, s>>>(in, H, W, C, out, out_split, Ho, Wo);
+  k_maxpool3s2_dense<<<device_sm_count() * 8, 256, 0, s>>>(in, H, W, C, out, out_split, Ho, Wo);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -301,7 +301,7 @@ __global__ void k_nearest_add_dense(float* __restrict__ fine, int Hf, int Wf, co
   }
 }
 int nearest_add_dense(float* fine, int Hf, int Wf, const float* coarse, int Hc, int Wc, int C, cudaStream_t s) {
-  k_nearest_add_dense<<<148 * 4, 256, 0, s>>>(fine, Hf, Wf, coarse, Hc, Wc, C, (float)Hc / (float)Hf, (float)Wc / (float)Wf);
+  k_nearest_add_dense<<<device_sm_count() * 4, 256, 0, s>>>(fine, Hf, Wf, coarse, Hc, Wc, C, (float)Hc / (float)Hf, (float)Wc / (float)Wf);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }

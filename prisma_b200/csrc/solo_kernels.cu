@@ -1,4 +1,4 @@
-// prisma_b200 -- SOLOv2 (mask_mmdet band) kernels outside the tcgen05 GEMM core: test-pipeline pre-process, the
+// prisma_b200 -- SOLOv2 (mask_mmdet band) kernels outside the wgmma GEMM core: test-pipeline pre-process, the
 // pooling / resampling glue of ResNet + FPN + SOLOV2Head, GroupNorm, and the whole decode (candidate selection, mask
 // statistics, Matrix NMS, the two chained bilinear resizes to the frame, the band's union mask).  Reference files are
 // cited per kernel (paths relative to bands/mmdet/).  All HBM- or latency-bound; nothing here is a GEMM.
@@ -98,7 +98,7 @@ __global__ void k_maxpool3s2(const __half* __restrict__ in, int H, int W, int C,
   }
 }
 int maxpool3s2_f16(const __half* in, int H, int W, int C, __half* out, int Ho, int Wo, cudaStream_t s) {
-  k_maxpool3s2<<<148 * 8, 256, 0, s>>>(in, H, W, C, out, Ho, Wo);
+  k_maxpool3s2<<<device_sm_count() * 8, 256, 0, s>>>(in, H, W, C, out, Ho, Wo);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -126,7 +126,7 @@ __global__ void k_nearest_add(__half* __restrict__ fine, int Hf, int Wf, const _
   }
 }
 int nearest_add_f16(__half* fine, int Hf, int Wf, const __half* coarse, int Hc, int Wc, int C, cudaStream_t s) {
-  k_nearest_add<<<148 * 4, 256, 0, s>>>(fine, Hf, Wf, coarse, Hc, Wc, C, (float)Hc / (float)Hf, (float)Wc / (float)Wf);
+  k_nearest_add<<<device_sm_count() * 4, 256, 0, s>>>(fine, Hf, Wf, coarse, Hc, Wc, C, (float)Hc / (float)Hf, (float)Wc / (float)Wf);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -207,7 +207,7 @@ int gn_stats(const float* x, int HW, int C, int groups, float* part, float* stat
 int groupnorm_relu_f16(const float* x, int H, int W, int C, int groups, const float* gamma, const float* beta, float* part,
                        float* stats, __half* out_padded, __half* out_dense, cudaStream_t s) {
   PRISMA_TRY(gn_stats(x, H * W, C, groups, part, stats, s));
-  k_gn_apply<<<148 * 4, 256, 0, s>>>(x, H, W, C, stats, gamma, beta, out_padded, out_dense);
+  k_gn_apply<<<device_sm_count() * 4, 256, 0, s>>>(x, H, W, C, stats, gamma, beta, out_padded, out_dense);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -298,7 +298,7 @@ __global__ void k_resize_bilinear(const __half* __restrict__ src, int Hs, int Ws
 }
 int resize_bilinear_f16(const __half* src, int Hs, int Ws, int Csrc, __half* dst, int Hd, int Wd, int Cdst, int coord,
                         int accumulate, cudaStream_t s, int dst_frame_w) {
-  k_resize_bilinear<<<148 * 4, 256, 0, s>>>(src, Hs, Ws, Csrc, dst, Hd, Wd, Cdst, (float)Hs / (float)Hd, (float)Ws / (float)Wd,
+  k_resize_bilinear<<<device_sm_count() * 4, 256, 0, s>>>(src, Hs, Ws, Csrc, dst, Hd, Wd, Cdst, (float)Hs / (float)Hd, (float)Ws / (float)Wd,
                                            coord, accumulate, dst_frame_w > 0 ? dst_frame_w : Wd);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -594,7 +594,7 @@ int solo_final_masks(const __half* masks, int fh, int fw, int h, int w, int H, i
                      const float* keep_score, const int* keep_label, const int* n_keep, int max_num, float confidence,
                      uint8_t* inst_masks, uint8_t* union_mask, cudaStream_t s) {
   (void)max_num;
-  k_solo_final<__half><<<148 * 8, 256, 0, s>>>(masks, fh, fw, h, w, H, W, mask_thr, keep, keep_score, keep_label, n_keep, confidence,
+  k_solo_final<__half><<<device_sm_count() * 8, 256, 0, s>>>(masks, fh, fw, h, w, H, W, mask_thr, keep, keep_score, keep_label, n_keep, confidence,
                                               (float)h / (float)H, (float)w / (float)W, inst_masks, union_mask);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -603,7 +603,7 @@ int solo_final_masks(const float* masks, int fh, int fw, int h, int w, int H, in
                      const float* keep_score, const int* keep_label, const int* n_keep, int max_num, float confidence,
                      uint8_t* inst_masks, uint8_t* union_mask, cudaStream_t s) {
   (void)max_num;
-  k_solo_final<float><<<148 * 8, 256, 0, s>>>(masks, fh, fw, h, w, H, W, mask_thr, keep, keep_score, keep_label, n_keep, confidence,
+  k_solo_final<float><<<device_sm_count() * 8, 256, 0, s>>>(masks, fh, fw, h, w, H, W, mask_thr, keep, keep_score, keep_label, n_keep, confidence,
                                              (float)h / (float)H, (float)w / (float)W, inst_masks, union_mask);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;

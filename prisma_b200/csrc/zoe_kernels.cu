@@ -1,6 +1,6 @@
 // prisma_b200 -- pointwise kernels of the ZoeDepth metric head on the Depth-Anything core (bands/depth_anything.py:106-119,
 // bands/patchfusion/zoedepth/models/zoedepth/zoedepth_v1.py:127-211).  Everything GEMM-shaped (the 1x1 convs of the
-// projectors / regressors / attractor MLPs) runs on the tcgen05 core; these are the HBM-bound pieces in between.
+// projectors / regressors / attractor MLPs) runs on the wgmma core; these are the HBM-bound pieces in between.
 #include "zoe_kernels.cuh"
 
 #include <math.h>
@@ -71,7 +71,7 @@ __global__ void k_zoe_embed_add(const float* __restrict__ a, int H, int W, int C
   }
 }
 int zoe_embed_add(const float* a, int H, int W, int C, const float* prev, int Hp, int Wp, __half* out, cudaStream_t s) {
-  k_zoe_embed_add<<<148 * 4, 256, 0, s>>>(a, H, W, C, prev, Hp, Wp, H > 1 ? (float)(Hp - 1) / (H - 1) : 0.f,
+  k_zoe_embed_add<<<device_sm_count() * 4, 256, 0, s>>>(a, H, W, C, prev, Hp, Wp, H > 1 ? (float)(Hp - 1) / (H - 1) : 0.f,
                                          W > 1 ? (float)(Wp - 1) / (W - 1) : 0.f, out);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -101,7 +101,7 @@ __global__ void k_zoe_attractor(const float* __restrict__ A, int lda, int n_attr
 }
 int zoe_attractor(const float* A, int lda, int n_attr, const float* b_prev, int Hp, int Wp, int H, int W, int bins, float* b_out,
                   cudaStream_t s) {
-  k_zoe_attractor<<<148 * 4, 256, 0, s>>>(A, lda, n_attr, b_prev, Hp, Wp, H, W, bins, H > 1 ? (float)(Hp - 1) / (H - 1) : 0.f,
+  k_zoe_attractor<<<device_sm_count() * 4, 256, 0, s>>>(A, lda, n_attr, b_prev, Hp, Wp, H, W, bins, H > 1 ? (float)(Hp - 1) / (H - 1) : 0.f,
                                          W > 1 ? (float)(Wp - 1) / (W - 1) : 0.f, b_out);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -136,7 +136,7 @@ __global__ void k_zoe_concat(const __half* __restrict__ act32, const float* __re
   }
 }
 int zoe_concat(const __half* act32, const float* rel, const float* emb, int He, int We, int H, int W, __half* out, cudaStream_t s) {
-  k_zoe_concat<<<148 * 8, 256, 0, s>>>(act32, rel, emb, He, We, H, W, H > 1 ? (float)(He - 1) / (H - 1) : 0.f,
+  k_zoe_concat<<<device_sm_count() * 8, 256, 0, s>>>(act32, rel, emb, He, We, H, W, H > 1 ? (float)(He - 1) / (H - 1) : 0.f,
                                       W > 1 ? (float)(We - 1) / (W - 1) : 0.f, out);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -181,7 +181,7 @@ __global__ void k_zoe_final(const float* __restrict__ pt, const float* __restric
 int zoe_final(const float* pt, const float* centers, int Hc, int Wc, int H, int W, int bins, float min_temp, float max_temp,
               float* out, cudaStream_t s) {
   PRISMA_CHECK(bins == 64, "zoe: 64 bins expected");
-  k_zoe_final<<<148 * 8, 256, 0, s>>>(pt, centers, Hc, Wc, H, W, H > 1 ? (float)(Hc - 1) / (H - 1) : 0.f,
+  k_zoe_final<<<device_sm_count() * 8, 256, 0, s>>>(pt, centers, Hc, Wc, H, W, H > 1 ? (float)(Hc - 1) / (H - 1) : 0.f,
                                      W > 1 ? (float)(Wc - 1) / (W - 1) : 0.f, min_temp, max_temp, out);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -234,8 +234,8 @@ __global__ void k_pil_v(const float* __restrict__ tmp, int ih, int ow, float* __
   }
 }
 int pil_bicubic_resize_f32(const float* in, int ih, int iw, float* tmp, float* out, int oh, int ow, cudaStream_t s) {
-  k_pil_h<<<148 * 8, 256, 0, s>>>(in, ih, iw, tmp, ow, (double)iw / (double)ow);
-  k_pil_v<<<148 * 8, 256, 0, s>>>(tmp, ih, ow, out, oh, (double)ih / (double)oh);
+  k_pil_h<<<device_sm_count() * 8, 256, 0, s>>>(in, ih, iw, tmp, ow, (double)iw / (double)ow);
+  k_pil_v<<<device_sm_count() * 8, 256, 0, s>>>(tmp, ih, ow, out, oh, (double)ih / (double)oh);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -123,8 +123,7 @@ class SoloV2Lanes:
     """The video loop of the band (mask_mmdet.py:131-154) over several engines at once: frames are independent, so `lanes`
     engines (one handle, stream, CUDA graph and set of plan buffers each; a handle is not re-entrant) take consecutive frames
     from worker threads -- the C calls release the GIL -- and the GPU overlaps the passes: one frame's ~200 short launches no
-    longer leave the SMs idle between kernels (B200, 1080p, host frame -> host union mask: 105 -> 154 frames/s with the fp32-class
-    head, 172 -> 322 with the fp16 head, 1 -> 4 lanes).  Results come back in frame order and are the same as SoloV2Engine.infer's."""
+    longer leave the SMs idle between kernels.  Results come back in frame order and are the same as SoloV2Engine.infer's."""
 
     def __init__(self, state_dict, device=0, variant="r101", lanes=4):
         from concurrent.futures import ThreadPoolExecutor

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """PRISMA orchestrator -- the reference's process.py surface (flags :76-99, defaults :18-56, band order :163-290) on top
-of the B200 bands.
+of the H100 bands.
 
     python process.py -i clip.mp4 [-d depth_anything|depth_midas|...|all] [-f flow_raft|flow_gmflow|all] [-e N] [-b] [-m] ...
 
@@ -52,7 +52,7 @@ def run(band, input_folder, output_file="", subpath=False, extra_args=""):
     """reference process.py:60-73, with subprocess instead of os.system so a failing band is reported."""
     print("\n# ", band.upper())
     if band not in ACCELERATED:
-        print(f"[process] band '{band}' is outside the B200 hot path (SURVEY.md section 8): skipped")
+        print(f"[process] band '{band}' is outside the H100 hot path (SURVEY.md section 8): skipped")
         return 1
     cmd = [sys.executable, os.path.join(ROOT, "bands", band + ".py"), "-i", input_folder]
     if output_file != "":
@@ -165,7 +165,7 @@ def main(argv=None):
     if args.depth is None:
         args.depth = DEPTH_VIDEO_DEFAULT if video else DEPTH_IMAGE_DEFAULT
         if args.depth not in ACCELERATED:
-            print(f"[process] the reference's default depth band for this input ({args.depth}) is outside the B200 hot "
+            print(f"[process] the reference's default depth band for this input ({args.depth}) is outside the H100 hot "
                   f"path; running depth_anything instead")
             args.depth = "depth_anything"
     ran_depth = []
@@ -193,7 +193,7 @@ def main(argv=None):
         if args.flow is None:
             args.flow = FLOW_DEFAULT
             if args.flow not in ACCELERATED:
-                print(f"[process] the reference's default flow band ({args.flow}) is outside the B200 hot path; running "
+                print(f"[process] the reference's default flow band ({args.flow}) is outside the H100 hot path; running "
                       f"flow_raft instead")
                 args.flow = "flow_raft"
         flow_args = ("--backwards " if args.flow_backwards else "") + ("--mask " if args.flow_mask else "")

@@ -1,8 +1,7 @@
 #!/bin/bash
 # Runs every -m gpu test file in its own process (a trapped kernel poisons only its own CUDA context),
-# each under a hard timeout so a protocol bug can never hang the GPU box.
+# each under a hard timeout so a protocol bug can never hang the GPU.
 cd "$(dirname "$0")/.."
-mkdir -p gpurun_out
 rc=0
 for f in tests/test_*_gpu.py tests/test_band_surface.py; do
   echo "=== $f"

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 attention kernel vs torch softmax attention (attention.py:49-62 semantics)."""
+"""GPU: wgmma attention kernel vs torch softmax attention (attention.py:49-62 semantics)."""
 import ctypes as C
 
 import numpy as np

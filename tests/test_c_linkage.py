@@ -1,5 +1,5 @@
 """The drop-in boundary is a C ABI: a plain-C client (examples/c_abi_minimal.c) compiles against include/prisma_b200.h,
-links libprisma_b200.so and runs without Python or torch in the process.  On a machine without a B200 it also shows
+links libprisma_b200.so and runs without Python or torch in the process.  On a machine without an H100 it also shows
 that engine creation fails loudly (negative code + message) instead of falling back."""
 import os
 import subprocess

@@ -54,8 +54,8 @@ def test_depth_band_matches_reference_fixture(golden_dir, vits_engine, tag):
     assert max(report["minmax"]) <= TOL
     # the u8 heat frame (what the band writes into <band>.mp4) against the REFERENCE's frame.  heat_to_rgb has slope
     # 6 * 0.65 per unit of normalised depth (encode.py:13-33), so an error e of the normalised depth moves a channel by at
-    # most 255 * 3.9 * e before the truncating cast: the frame may differ by the propagated float error only.  Measured on
-    # B200: max 1 LSB, mean 0.06 LSB (normalised-depth error ~1e-3: the seeded weights span only 0.236..0.280).
+    # most 255 * 3.9 * e before the truncating cast: the frame may differ by the propagated float error only (the seeded weights span
+    # only 0.236..0.280 of depth, so a 1e-3 normalised-depth error is a few LSB at most).
     span = float(g["dmax"]) - float(g["dmin"])
     e_norm = (float(np.abs(pred - g["prediction"]).max()) + 2 * max(report["minmax"]) * float(g["dmax"])) / span
     lsb_bound = int(np.ceil(255 * 3.9 * e_norm)) + 1

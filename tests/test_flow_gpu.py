@@ -22,8 +22,8 @@ def test_raft_preprocess(H, W, kind):
     re-derived from the rounded output size).  The 8-bit cubic of this OpenCV build is IPP's float pipeline, round half to
     even; the kernel is byte-equal to it except at exact .5 ties of the real-valued result, where IPP's closed, CPU-
     dispatched operation order decides: every differing byte must be such a tie (|exact - (n + .5)| < 1e-4, the float32
-    rounding noise of a 16-tap sum of values up to 255), by 1 LSB.  Measured on B200: 1e-5 of the bytes on uniform noise,
-    5e-4 on the smooth synthetic frames (flat regions make exact ties common); bound 1e-3.  Padding / normalisation are exact."""
+    rounding noise of a 16-tap sum of values up to 255), by 1 LSB.  Flat regions make exact ties common on the
+    smooth synthetic frames; bound 1e-3 of the bytes.  Padding / normalisation are exact."""
     img = synthetic_frame(H, W, 2) if kind == "synthetic" else np.random.default_rng(H).integers(0, 256, (H, W, 3), dtype=np.uint8)
     ref_rs = oraft.raft_preprocess(img)  # 3 x hs x ws float (0..255), via cv2
     hs, ws = ref_rs.shape[-2:]

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 shifted-row GEMM core through the C ABI vs a plain fp32 reference on fp16-rounded operands."""
+"""GPU: the wgmma shifted-row GEMM core through the C ABI vs a plain fp32 reference on fp16-rounded operands."""
 import ctypes as C
 
 import numpy as np
@@ -32,26 +32,26 @@ def _gemm(A, W, bias, act, bn):
     (1813, 1536, 384, 1, 64),    # BN=64, gelu
     (500, 48, 384, 0, 0),        # narrow N (ViT-S head), BN=32/64
     (333, 32, 1152, 2, 32),      # BN=32
-    (40000, 256, 128, 0, 0),     # many tiles per CTA (persistent loop, TMEM double buffering)
+    (40000, 256, 128, 0, 0),     # many tiles per CTA (persistent loop, operand ring wrapping across tiles)
     (64, 64, 64, 0, 0),          # smaller than a tile
-    (512, 256, 128, 0, 512),     # CTA pairs (cta_group::2, 256x256 tiles): one pair tile per pair
-    (2443, 3072, 1024, 0, 512),  # CTA pairs, ViT-L qkv: ragged M, many tiles per pair
-    (9772, 1024, 4096, 1, 512),  # CTA pairs, 4-frame fc2 shape with gelu
-    (300, 256, 200, 2, 512),     # CTA pairs: second CTA's rows partly / fully out of range, K tail
-    (37000, 128, 1920, 0, 384),  # CTA pairs with 256 x 128 tiles (the RAFT GRU q conv shape), ragged M
-    (700, 256, 320, 2, 384),     # 256 x 128 pair tiles, two column tiles, K tail
-    # auto tile choice with a partial last wave -> mixed-width tail tiles (GemmArgs::tail_split)
-    (29316, 1024, 192, 0, 0),    # CTA pairs: 460 pair tiles = 6 waves + 16 -> the 16 cut into 4 x 64-wide tiles
-    (26624, 256, 128, 2, 0),     # CTA pairs: 104 pair tiles = 1 wave + 30 -> cut into 2 x 128-wide tiles
-    (39008, 128, 384, 1, 0),     # single CTAs, 128-wide: 305 tiles = 2 waves + 9 -> 2 x 64-wide tiles, gelu
-    (20000, 64, 128, 0, 0),      # 64-wide: 157 tiles = 1 wave + 9 -> 2 x 32-wide tiles
-    # transposed tiles (GemmCfg SWAP, force 640): 128 output columns x 256 rows per instruction, epilogue transposed
-    (256, 128, 64, 0, 640),      # one tile, one k-block
-    (37000, 128, 1920, 0, 640),  # the RAFT GRU q conv shape: ragged M (the last tile has 136 valid rows), many tiles per CTA
-    (5000, 96, 576, 2, 640),     # N = 96 (RAFT encoder layer 2): the fourth column quarter is beyond N; relu
+    (512, 256, 128, 0, 512),     # force_bn 512 -> 256-wide tiles: four row tiles, one column tile
+    (2443, 3072, 1024, 0, 512),  # 256-wide tiles, ViT-L qkv: ragged M, several tiles per CTA
+    (9772, 1024, 4096, 1, 512),  # 256-wide tiles, 4-frame fc2 shape with gelu (long K: the operand ring wraps many times)
+    (300, 256, 200, 2, 512),     # 256-wide tiles: the last row tile's slabs partly / fully out of range, K tail
+    (37000, 128, 1920, 0, 384),  # force_bn 384 -> 128-wide tiles (the RAFT GRU q conv shape), ragged M
+    (700, 256, 320, 2, 384),     # 128-wide tiles, two column tiles, K tail
+    # auto tile choice (gemm_pick_bn) with a partial last wave
+    (29316, 1024, 192, 0, 0),    # ViT-L fc1-like rows, short K
+    (26624, 256, 128, 2, 0),     # relu, two 128-wide or one 256-wide column tile
+    (39008, 128, 384, 1, 0),     # 305 row tiles on 132 SMs (2.3 waves), gelu
+    (20000, 64, 128, 0, 0),      # narrow N: 157 row tiles
+    # force_bn 640 -> 128-wide tiles; N <= 128 shapes with ragged edges
+    (256, 128, 64, 0, 640),      # two row tiles, one k-block
+    (37000, 128, 1920, 0, 640),  # the RAFT GRU q conv shape: ragged M, many tiles per CTA
+    (5000, 96, 576, 2, 640),     # N = 96 (RAFT encoder layer 2): the last 32-column chunk is beyond N; relu
     (777, 128, 200, 1, 640),     # K tail, gelu, M not a multiple of 32
-    (151552, 128, 256, 0, 0),    # auto choice picks the transposed tiles (N <= 128, M >= 4096): 8 whole waves
-    (4100, 68, 128, 0, 640),     # N % 32 = 4: one 4-column group of the third quarter valid
+    (151552, 128, 256, 0, 0),    # auto choice, N = 128, 1184 row tiles: many tiles per CTA
+    (4100, 68, 128, 0, 640),     # N % 32 = 4: one 4-column group of the third 32-column chunk valid
 ])
 def test_gemm_matches_fp32_reference(M, N, K, act, bn):
     rng = np.random.default_rng(M * 7 + N * 3 + K)
@@ -70,13 +70,13 @@ def test_gemm_matches_fp32_reference(M, N, K, act, bn):
 
 
 @pytest.mark.parametrize("M,N,K,bn", [
-    (18360, 18360, 256, 0),   # RAFT correlation level 0 at 1080p x 0.75: CTA pairs, ragged M and N (N % 32 = 24)
+    (18360, 18360, 256, 0),   # RAFT correlation level 0 at 1080p x 0.75: ragged M and N (N % 32 = 24)
     (18360, 4592, 512, 0),    # level 1 (hi/lo pooled features: K = 512), N % 32 = 16
-    (1000, 264, 256, 128),    # level 3 size class, single CTAs, 128-wide tiles
-    (300, 520, 64, 256),      # single CTAs, 256-wide, rows of the last tile out of range
+    (1000, 264, 256, 128),    # level 3 size class, 128-wide tiles
+    (300, 520, 64, 256),      # 256-wide, rows of the last tile out of range
 ])
 def test_gemm_tma_store_epilogue(M, N, K, bn):
-    """The TMA-store epilogue (tcgen05.ld -> swizzled smem box -> cp.async.bulk.tensor store): dense fp32 output scaled by
+    """The TMA-store epilogue (accumulator registers -> swizzled smem box -> cp.async.bulk.tensor store): dense fp32 output scaled by
     1/16, boxes clipped at ragged M / N edges, nothing written outside [M][N]."""
     rng = np.random.default_rng(M + N + K)
     A = rng.standard_normal((M, K), dtype=np.float32)
@@ -90,13 +90,13 @@ def test_gemm_tma_store_epilogue(M, N, K, bn):
 
 
 @pytest.mark.parametrize("M,N,K,bn", [
-    (18360, 18360, 256, 0),   # RAFT correlation level 0 at 1080p x 0.75: CTA pairs, ragged M and N (N % 32 = 24)
+    (18360, 18360, 256, 0),   # RAFT correlation level 0 at 1080p x 0.75: ragged M and N (N % 32 = 24)
     (18360, 4592, 512, 0),    # level 1 (hi/lo pooled features: K = 512), N % 32 = 16
-    (1000, 264, 256, 128),    # level 3 size class, single CTAs, 128-wide tiles
-    (300, 520, 64, 256),      # single CTAs, 256-wide, rows of the last tile out of range
+    (1000, 264, 256, 128),    # level 3 size class, 128-wide tiles
+    (300, 520, 64, 256),      # 256-wide, rows of the last tile out of range
 ])
 def test_gemm_tma_store_epilogue_fp16(M, N, K, bn):
-    """The same epilogue with an fp16 destination (32 x 64-byte boxes, 64-byte swizzle): fp32 accumulate, scaled by 1/16,
+    """The same epilogue with an fp16 destination (32 x 128-byte boxes of 64 columns, 128-byte swizzle): fp32 accumulate, scaled by 1/16,
     rounded once; every element of [M][N] written (the buffer starts as NaN), boxes clipped at the ragged edges."""
     rng = np.random.default_rng(M + N + K + 1)
     A = rng.standard_normal((M, K), dtype=np.float32)
@@ -110,9 +110,9 @@ def test_gemm_tma_store_epilogue_fp16(M, N, K, bn):
 
 
 @pytest.mark.parametrize("M,N,K,act,bn", [
-    (29316, 4096, 1024, -6, 0),   # ViT-L fc1 at 12 frames: CTA pairs, ragged M, tail tiles, bias + GELU
+    (29316, 4096, 1024, -6, 0),   # ViT-L fc1 at 12 frames: ragged M, bias + GELU
     (2443, 3072, 1024, -7, 0),    # qkv-like, bias + ReLU
-    (700, 328, 200, -6, 128),     # single CTAs, N % 64 = 8: the last 64-column box is clipped to 8 columns, K tail
+    (700, 328, 200, -6, 128),     # N % 64 = 8: the last 64-column box is clipped to 8 columns, K tail
 ])
 def test_gemm_tma_store_epilogue_fp16_bias_activation(M, N, K, act, bn):
     """The fp16 TMA-store epilogue of the ViT qkv / fc1 linears: bias and GELU / ReLU applied in the row-per-lane registers,
@@ -131,8 +131,8 @@ def test_gemm_tma_store_epilogue_fp16_bias_activation(M, N, K, act, bn):
 
 
 @pytest.mark.parametrize("M,N,K,bn", [
-    (29316, 1024, 4096, 0),   # ViT-L fc2 at 12 frames: CTA pairs, ragged M
-    (2443, 384, 384, 0),      # ViT-S proj: single CTAs, 128-wide tiles
+    (29316, 1024, 4096, 0),   # ViT-L fc2 at 12 frames: ragged M
+    (2443, 384, 384, 0),      # ViT-S proj, 128-wide tiles
     (300, 264, 200, 128),     # ragged N (N % 32 = 8), K tail
 ])
 def test_gemm_tma_reduce_epilogue_in_place_residual(M, N, K, bn):
@@ -176,11 +176,10 @@ def test_conv_matches_torch(H, W, Cin, Cout, k, relu):
 
 @pytest.mark.parametrize("M,N,K,bn", [(300, 256, 512, 0), (4096, 512, 2304, 0), (1600, 80, 4608, 0), (5000, 128, 320, 128), (64, 32, 100, 32)])
 def test_gemm_tf32x3_is_fp32_class(M, N, K, bn):
-    """The 3xTF32 path (kind::tf32 MMAs on [hi | lo] splits of both operands) against the exact product (float64).  The
+    """The 3xTF32 path (tf32 MMAs on [hi | lo] splits of both operands) against the exact product (float64).  The
     products are fp32-class (the dropped lo x lo term is 2^-22).  The tensor core's own fp32 ACCUMULATION truncates the aligned
-    addends instead of rounding them -- with the whole K in one TMEM chain that bias measured 3e-6 .. 6e-6 of sum |a||w| on
-    B200 (growing with K; PRISMA_TF32_ACC_GROUP=0 reproduces it), i.e. only 1e-4-class results for K ~ 4600.  The kernel
-    therefore keeps a TMEM chain 4 K-blocks (16 MMAs) long and adds the partial sums in registers with round-to-nearest
+    addends instead of rounding them, a bias that grows with K (PRISMA_TF32_ACC_GROUP=0 reproduces it).  The kernel
+    therefore keeps a wgmma chain 4 K-blocks (16 MMAs) long and adds the partial sums in registers with round-to-nearest
     FADDs (GemmArgs::acc_group): the error is then that of a CUDA-core fp32 GEMM."""
     rng = np.random.default_rng(M + N + K)
     A = (rng.standard_normal((M, K), dtype=np.float32) * rng.uniform(0.01, 30.0, (M, 1)).astype(np.float32))

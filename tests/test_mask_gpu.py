@@ -118,14 +118,11 @@ def test_solo_tiny_stages_and_results(tiny):
 def test_solo_head_and_decode_from_the_reference_levels_reproduce_the_reference_instances(tiny, golden_dir):
     """north_star: mask ids bit-exact.  tests/golden/solo_tiny_head.npz holds the VENDORED mmdet SOLOV2Head's own FPN
     levels and its final scores / labels / masks (oracle/tools/make_golden.py).  Replaying head + decode from those levels
-    on the fp32-class path (three kind::tf32 tensor-core passes per contraction, fp32 activations) must give the same
+    on the fp32-class path (three tf32 tensor-core passes per contraction, fp32 activations) must give the same
     instance list: the same labels in the same order, scores to 5e-5 relative, masks bit-equal except razor-margin boundary
-    pixels (|p - 0.5| ~ 1e-6), at most 1e-6 of the bits.  Measured on B200: labels equal, scores 6.4e-6, 3 of 7.68 M mask
-    bits (an exact-arithmetic emulation of 3xTF32 in the oracle: 1.5e-6 and 1 bit; two fp32 implementations that sum in a
-    different order -- cuDNN vs MKL-DNN -- differ the same way).  Getting there needed the external fp32 accumulation of
-    gemm_prepare_tf32x3: with whole-K TMEM chains the tensor core's truncating accumulate left 4.6e-4 on the class logits,
-    swapped two ranks and moved scores by 2e-3.  The single-pass fp16 head of round 1 changes a third of the list on the
-    same input (labels differ, scores off by 2e-3, 4 % of the mask bits)."""
+    pixels (|p - 0.5| ~ 1e-6), at most 1e-6 of the bits (two fp32 implementations that sum in a different order differ
+    the same way).  This needs the external fp32 accumulation of gemm_prepare_tf32x3: with whole-K accumulation chains the
+    tensor core's truncating accumulate moves the class logits enough to swap ranks."""
     import os
     eng, sd = tiny
     g = np.load(os.path.join(golden_dir, "solo_tiny_head.npz"))
