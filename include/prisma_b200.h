@@ -207,10 +207,57 @@ int prisma_net_size(const char* band, int w, int h, int* wn, int* hn);
 
 /* ---- kernel-level entry points (parity tests and micro-benchmarks call the kernels through the C ABI) ---- */
 /* D = A[M,K] * W[N,K]^T (+bias) with fp16 operands / fp32 accumulate on the wgmma core; A, W, D host fp32.
- * act: 0 none, 1 gelu, 2 relu; -4 = the TMA-store epilogue (no bias, accumulator scaled by 1/16: the RAFT correlation path).
+ * act: 0 none, 1 gelu, 2 relu (register epilogue, fp32 out); TMA-store epilogues: -4 fp32 out, no bias, accumulator scaled
+ * by 1/16 (the RAFT correlation path); -5 the same with an fp16 destination; -6 / -7 fp16 out with bias + GELU / ReLU (the
+ * ViT qkv / fc1 path); -8 D (zeros) += acc + bias in place through the TMA reduce-add, once per launch.
  * force_bn: 0 = auto, else 32/64/128/256 (512 / 384 / 640: the 256- / 128-wide tiles).  ms_out (may be NULL): kernel time.                               */
 int prisma_debug_gemm(int device, const float* A, const float* W, const float* bias, float* D, int M, int N, int K,
                       int act, int force_bn, int iters, float* ms_out);
+/* The fused GEMM epilogue (prisma_b200/csrc/gemm_tc.cuh, GemmEpilogue) as a C struct: every field a caller sets, with the
+ * same meaning and the same defaults (alpha 1, sub 1, pad 1, out_pad 1, lead -1, out_lead -1, shuf_s 1, everything else 0).
+ * `size` must be sizeof(prisma_debug_epilogue).  All pointers are DEVICE pointers; the fp16 ones point at IEEE binary16.   */
+typedef struct prisma_debug_epilogue {
+  int size;
+  float alpha;
+  const float* bias;
+  const float* gamma;
+  int act;                       /* 0 none, 1 GELU, 2 ReLU, 3 sigmoid, 4 tanh (fast), 5 softplus, 6 sigmoid (IEEE)        */
+  const float* pre_f32;
+  int pre_f32_ld;
+  const float* res_f32;
+  int res_f32_ld;
+  const void* res_a;
+  int res_a_ld;
+  const void* res_b;
+  int res_b_ld;
+  float* out_f32;
+  int out_f32_ld;
+  void* out_f16;
+  int out_f16_ld;
+  void* out_f16_relu;
+  int out_f16_relu_ld;
+  int row_map;                   /* 0 LINEAR, 1 PADDED, 2 TOK2PAD, 3 SHUFFLE, 4 TOKSKIP, 5 PAD2TOK                        */
+  int img_rows, in_w, in_h, out_wp, out_img_rows, sub, pad, out_pad, lead, out_lead, shuf_s, shuf_cout;
+  const float* head_w;
+  float head_b;
+  float* head_out;
+  float* stat_part;
+  const int* m_dev;
+  int tma_store;
+  int gru;
+  const float* gru_h;
+  const float* gru_z;
+  void* gru_rh;
+  int gru_rh_ld;
+} prisma_debug_epilogue;
+/* One launch of the shifted-row GEMM  D[m, n] = sum_t sum_c A[m + tap_off[t], c] W[n, t * round_up(a_cols, 64) + c]
+ * with the epilogue `ep`, on caller-owned DEVICE buffers, on stream 0, then a device synchronise.
+ * tf32 == 0: A fp16 [a_rows][a_pitch] (a_cols used), W fp16 [w_rows][taps * round_up(a_cols, 64)].
+ * tf32 != 0: the 3xTF32 path; A fp32 [a_rows][2 * c_half] = [hi | lo] (a_pitch == 2 * c_half; a_cols = C channels used),
+ * W fp32 [w_rows][taps * 3 * C] = per tap [hi | hi | lo].  force_bn: 0 = auto, else 32/64/128/256.                         */
+int prisma_debug_gemm_ep(int device, const void* A, long long a_rows, int a_cols, int a_pitch, const void* W, int w_rows,
+                         int M, int N, int taps, const int* tap_off, int force_bn, int tf32, int c_half,
+                         const prisma_debug_epilogue* ep);
 /* The same product through the 3xTF32 path of the mask band (kind::tf32 tensor-core MMAs on [hi | lo] splits of both
  * operands: fp32-class products, ~1e-6 relative): D = A W^T + bias, all fp32.                                  */
 int prisma_debug_gemm_tf32x3(int device, const float* A, const float* W, const float* bias, float* D, int M, int N, int K,

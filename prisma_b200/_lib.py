@@ -15,6 +15,28 @@ c_u8_p = C.POINTER(C.c_uint8)
 c_i64_p = C.POINTER(C.c_int64)
 c_double_p = C.POINTER(C.c_double)
 
+
+class DebugEpilogue(C.Structure):
+    """Mirror of `prisma_debug_epilogue` (include/prisma_b200.h): pointer fields take device addresses (ints)."""
+    _fields_ = [
+        ("size", C.c_int), ("alpha", C.c_float), ("bias", C.c_void_p), ("gamma", C.c_void_p), ("act", C.c_int),
+        ("pre_f32", C.c_void_p), ("pre_f32_ld", C.c_int), ("res_f32", C.c_void_p), ("res_f32_ld", C.c_int),
+        ("res_a", C.c_void_p), ("res_a_ld", C.c_int), ("res_b", C.c_void_p), ("res_b_ld", C.c_int),
+        ("out_f32", C.c_void_p), ("out_f32_ld", C.c_int), ("out_f16", C.c_void_p), ("out_f16_ld", C.c_int),
+        ("out_f16_relu", C.c_void_p), ("out_f16_relu_ld", C.c_int),
+        ("row_map", C.c_int), ("img_rows", C.c_int), ("in_w", C.c_int), ("in_h", C.c_int), ("out_wp", C.c_int),
+        ("out_img_rows", C.c_int), ("sub", C.c_int), ("pad", C.c_int), ("out_pad", C.c_int), ("lead", C.c_int),
+        ("out_lead", C.c_int), ("shuf_s", C.c_int), ("shuf_cout", C.c_int),
+        ("head_w", C.c_void_p), ("head_b", C.c_float), ("head_out", C.c_void_p), ("stat_part", C.c_void_p),
+        ("m_dev", C.c_void_p), ("tma_store", C.c_int),
+        ("gru", C.c_int), ("gru_h", C.c_void_p), ("gru_z", C.c_void_p), ("gru_rh", C.c_void_p), ("gru_rh_ld", C.c_int),
+    ]
+
+    def __init__(self, **kw):
+        defaults = dict(size=C.sizeof(DebugEpilogue), alpha=1.0, sub=1, pad=1, out_pad=1, lead=-1, out_lead=-1, shuf_s=1)
+        defaults.update(kw)
+        super().__init__(**defaults)
+
 # name -> (restype, argtypes); must list every symbol declared in include/prisma_b200.h
 SIGNATURES = {
     "prisma_last_error": (C.c_char_p, []),
@@ -78,6 +100,8 @@ SIGNATURES = {
                                     C.c_int, C.c_int, C.c_int, c_float_p]),
     "prisma_debug_gemm_tf32x3": (C.c_int, [C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int,
                                            C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_gemm_ep": (C.c_int, [C.c_int, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int, C.POINTER(DebugEpilogue)]),
     "prisma_debug_conv": (C.c_int, [C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
     "prisma_debug_attention": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p]),

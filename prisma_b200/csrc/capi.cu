@@ -244,18 +244,13 @@ int prisma_debug_gemm(int device, const float* A, const float* W, const float* b
   PRISMA_CUDA_OK(cudaMemcpy(dA, hA.data(), hA.size() * 2, cudaMemcpyHostToDevice));
   PRISMA_CUDA_OK(cudaMemcpy(dW, hW.data(), hW.size() * 2, cudaMemcpyHostToDevice));
   if (bias) PRISMA_CUDA_OK(cudaMemcpy(dB, bias, N * 4, cudaMemcpyHostToDevice));
+  PRISMA_CHECK((act >= 0 && act <= 2) || (act >= -8 && act <= -4), "debug gemm: act must be 0..2 or -4..-8");
   GemmEpilogue ep;
   ep.bias = bias ? dB : nullptr;
   ep.act = act < 0 ? 0 : act;
-  ep.out_f32 = act == -1 ? nullptr : dD;  // act == -1: mainloop only (no stores), act == -2: fp16 output
+  ep.out_f32 = dD;
   ep.out_f32_ld = N;
   __half* dH = nullptr;
-  if (act == -2) {
-    dH = sc.alloc<__half>((size_t)M * N);
-    ep.out_f32 = nullptr;
-    ep.out_f16 = dH;
-    ep.out_f16_ld = N;
-  }
   if (act == -4) {  // TMA-store epilogue (dense fp32, scaled)
     ep.bias = nullptr;
     ep.alpha = 0.0625f;
@@ -288,11 +283,6 @@ int prisma_debug_gemm(int device, const float* A, const float* W, const float* b
     ep.res_f32 = dD;
     ep.res_f32_ld = N;
     ep.tma_store = true;
-    PRISMA_CUDA_OK(cudaMemset(dD, 0, (size_t)M * N * 4));
-  }
-  if (act == -3) {  // micro-benchmark of the residual-stream epilogue: D += acc in place (fp32 read + write)
-    ep.res_f32 = dD;
-    ep.res_f32_ld = N;
     PRISMA_CUDA_OK(cudaMemset(dD, 0, (size_t)M * N * 4));
   }
   GemmLaunch g;
@@ -351,6 +341,63 @@ int prisma_debug_gemm_tf32x3(int device, const float* A, const float* W, const f
   PRISMA_TRY(gemm_prepare_tf32x3(&g, dA, M, C, C, dW, Nw, M, N, 1, off, ep, sms, force_bn));
   PRISMA_TRY(timed(0, iters > 0 ? iters : 1, ms_out, [&]() { return gemm_run(g, 0); }));
   PRISMA_CUDA_OK(cudaMemcpy(Dout, dD, (size_t)M * N * 4, cudaMemcpyDeviceToHost));
+  return 0;
+  API_GUARD_END
+}
+
+// One prepared launch of the shifted-row GEMM with a caller-described epilogue, on caller-owned device buffers (stream 0),
+// followed by a device synchronise.  Every field of GemmEpilogue except tma_reduce (derived by gemm_prepare) is settable.
+int prisma_debug_gemm_ep(int device, const void* A, long long a_rows, int a_cols, int a_pitch, const void* W, int w_rows,
+                         int M, int N, int taps, const int* tap_off, int force_bn, int tf32, int c_half,
+                         const prisma_debug_epilogue* e) {
+  API_GUARD_BEGIN
+  PRISMA_CHECK(e != nullptr && tap_off != nullptr, "null argument");
+  PRISMA_CHECK(e->size == (int)sizeof(prisma_debug_epilogue), "prisma_debug_epilogue: size field does not match the library's struct");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  GemmEpilogue ep;
+  ep.alpha = e->alpha;
+  ep.bias = e->bias;
+  ep.gamma = e->gamma;
+  ep.act = e->act;
+  ep.pre_f32 = e->pre_f32; ep.pre_f32_ld = e->pre_f32_ld;
+  ep.res_f32 = e->res_f32; ep.res_f32_ld = e->res_f32_ld;
+  ep.res_a = static_cast<const __half*>(e->res_a); ep.res_a_ld = e->res_a_ld;
+  ep.res_b = static_cast<const __half*>(e->res_b); ep.res_b_ld = e->res_b_ld;
+  ep.out_f32 = e->out_f32; ep.out_f32_ld = e->out_f32_ld;
+  ep.out_f16 = static_cast<__half*>(e->out_f16); ep.out_f16_ld = e->out_f16_ld;
+  ep.out_f16_relu = static_cast<__half*>(e->out_f16_relu); ep.out_f16_relu_ld = e->out_f16_relu_ld;
+  ep.row_map = e->row_map;
+  ep.img_rows = e->img_rows;
+  ep.in_w = e->in_w;
+  ep.in_h = e->in_h;
+  ep.out_wp = e->out_wp;
+  ep.out_img_rows = e->out_img_rows;
+  ep.sub = e->sub;
+  ep.pad = e->pad;
+  ep.out_pad = e->out_pad;
+  ep.lead = e->lead;
+  ep.out_lead = e->out_lead;
+  ep.shuf_s = e->shuf_s;
+  ep.shuf_cout = e->shuf_cout;
+  ep.head_w = e->head_w; ep.head_b = e->head_b; ep.head_out = e->head_out;
+  ep.stat_part = e->stat_part;
+  ep.m_dev = e->m_dev;
+  ep.tma_store = e->tma_store != 0;
+  ep.gru = e->gru;
+  ep.gru_h = e->gru_h; ep.gru_z = e->gru_z;
+  ep.gru_rh = static_cast<__half*>(e->gru_rh); ep.gru_rh_ld = e->gru_rh_ld;
+  GemmLaunch g;
+  if (tf32) {
+    PRISMA_CHECK(a_pitch == 2 * c_half, "debug gemm_ep: a tf32 [hi | lo] operand has a row pitch of 2 * c_half");
+    PRISMA_TRY(gemm_prepare_tf32x3(&g, static_cast<const float*>(A), a_rows, a_cols, c_half, static_cast<const float*>(W), w_rows,
+                                   M, N, taps, tap_off, ep, sms, force_bn));
+  } else {
+    PRISMA_TRY(gemm_prepare(&g, static_cast<const __half*>(A), a_rows, a_cols, a_pitch, static_cast<const __half*>(W), w_rows,
+                            M, N, taps, tap_off, ep, sms, force_bn));
+  }
+  PRISMA_TRY(gemm_run(g, 0));
+  PRISMA_CUDA_OK(cudaDeviceSynchronize());
   return 0;
   API_GUARD_END
 }

@@ -171,6 +171,15 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
   out->args.acc_group = 1;
   const int bke = tf32 ? 32 : 64;  // elements per 128-byte K block
   PRISMA_CHECK(bn == 32 || bn == 64 || bn == 128 || bn == 256, "gemm: unsupported BLOCK_N");
+  // preconditions of the fused epilogues (without them the kernel writes wrong cells without any error)
+  PRISMA_CHECK(ep.row_map != ROW_SHUFFLE ||
+                   (ep.shuf_s >= 1 && ep.shuf_cout > 0 && ep.shuf_cout % 4 == 0 && N == ep.shuf_s * ep.shuf_s * ep.shuf_cout),
+               "gemm: ROW_SHUFFLE needs shuf_cout % 4 == 0 (a lane's 4 columns share one sub-pixel) and N == shuf_s^2 * shuf_cout");
+  PRISMA_CHECK(!ep.head_w || (N == 32 && ep.bias && ep.head_out && ep.row_map == ROW_PADDED && ep.lead < 0 && ep.sub == 1),
+               "gemm: the fused head needs N == 32, a bias, head_out and a stride-1 ROW_PADDED map with a symmetric border");
+  PRISMA_CHECK(ep.gru == 0 || (!tf32 && ep.gru_h &&
+                               ((ep.gru == 1 && N == 256 && ep.gru_rh) || (ep.gru == 2 && N == 128 && ep.gru_z))),
+               "gemm: the ConvGRU epilogue needs the fp16 path, gru_h, and N == 256 + gru_rh (gru 1) or N == 128 + gru_z (gru 2)");
   PRISMA_CHECK(w_rows >= round_up(N, bn), "gemm: weight rows must be padded to a multiple of BLOCK_N");
   const int kchunks = ceil_div(a_cols, bke);
   out->bn = bn;

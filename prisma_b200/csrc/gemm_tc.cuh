@@ -350,15 +350,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
-  const int M_run = args.ep.m_dev ? min(args.M, (*args.ep.m_dev + GEMM_BM - 1) / GEMM_BM * GEMM_BM) : args.M;  // see GemmEpilogue::m_dev
-  const int tiles_m = (M_run + GEMM_BM - 1) / GEMM_BM;
-  const int tiles_n = (args.N + BN - 1) / BN;
-  const int num_tiles = tiles_m * tiles_n;
-  const int num_kb = args.taps * args.kchunks;
-  auto tile_mn = [&](int tile, int* tm, int* tn) {
-    *tm = args.raster_n ? tile / tiles_n : tile % tiles_m;
-    *tn = args.raster_n ? tile % tiles_n : tile / tiles_m;
-  };
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
@@ -368,6 +359,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   __syncthreads();
   pdl_wait();  // barriers and descriptors are set up; from here on the predecessor's results are read
+
+  // *m_dev is written by the previous kernel (the SOLOv2 candidate count), so it is read only after the wait
+  const int M_run = args.ep.m_dev ? min(args.M, (*args.ep.m_dev + GEMM_BM - 1) / GEMM_BM * GEMM_BM) : args.M;  // see GemmEpilogue::m_dev
+  const int tiles_m = (M_run + GEMM_BM - 1) / GEMM_BM;
+  const int tiles_n = (args.N + BN - 1) / BN;
+  const int num_tiles = tiles_m * tiles_n;
+  const int num_kb = args.taps * args.kchunks;
+  auto tile_mn = [&](int tile, int* tm, int* tn) {
+    *tm = args.raster_n ? tile / tiles_n : tile % tiles_m;
+    *tn = args.raster_n ? tile % tiles_n : tile / tiles_m;
+  };
 
   if (wg == 2) {
     // ------------------------------------------------------------------ TMA producer
