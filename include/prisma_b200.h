@@ -140,8 +140,8 @@ int prisma_flow_infer_stream(prisma_engine* e, const uint8_t* frames, int n, int
                              int continue_clip, float* fwd, float* bwd, uint8_t* fwd_rgb, uint8_t* bwd_rgb, float* max_fwd,
                              float* max_bwd, int* pairs_out);
 /* Frame pairs per pass of the clip path (prisma_flow_infer_stream / _infer_resident / _work_detail / _profile): 1..4
- * (default 4; PRISMA_RAFT_PAIRS in the environment overrides; lowered per frame size until the correlation pyramids of one
- * pass fit in a third of the device memory -- 4K frames run one pair per pass).  With n, one pass takes n + 1 consecutive frames and
+ * (default 4; lowered per frame size until the correlation pyramids of one pass fit in a third of the device memory --
+ * 4K frames run one pair per pass).  With n, one pass takes n + 1 consecutive frames and
  * produces both directions of the n pairs: every update-block launch covers n times the rows, so the per-launch fixed
  * cost is shared by n pairs.  Results per pair are the same.  The pair calls prisma_flow_infer / _infer_video always use 1.   */
 int prisma_flow_set_pairs_per_pass(prisma_engine* e, int pairs);
@@ -210,7 +210,7 @@ int prisma_net_size(const char* band, int w, int h, int* wn, int* hn);
  * act: 0 none, 1 gelu, 2 relu (register epilogue, fp32 out); TMA-store epilogues: -4 fp32 out, no bias, accumulator scaled
  * by 1/16 (the RAFT correlation path); -5 the same with an fp16 destination; -6 / -7 fp16 out with bias + GELU / ReLU (the
  * ViT qkv / fc1 path); -8 D (zeros) += acc + bias in place through the TMA reduce-add, once per launch.
- * force_bn: 0 = auto, else 32/64/128/256 (512 / 384 / 640: the 256- / 128-wide tiles).  ms_out (may be NULL): kernel time.                               */
+ * force_bn: 0 = auto, else 32/64/128/256.  ms_out (may be NULL): kernel time.                                              */
 int prisma_debug_gemm(int device, const float* A, const float* W, const float* bias, float* D, int M, int N, int K,
                       int act, int force_bn, int iters, float* ms_out);
 /* The fused GEMM epilogue (prisma_b200/csrc/gemm_tc.cuh, GemmEpilogue) as a C struct: every field a caller sets, with the
@@ -254,7 +254,8 @@ typedef struct prisma_debug_epilogue {
  * with the epilogue `ep`, on caller-owned DEVICE buffers, on stream 0, then a device synchronise.
  * tf32 == 0: A fp16 [a_rows][a_pitch] (a_cols used), W fp16 [w_rows][taps * round_up(a_cols, 64)].
  * tf32 != 0: the 3xTF32 path; A fp32 [a_rows][2 * c_half] = [hi | lo] (a_pitch == 2 * c_half; a_cols = C channels used),
- * W fp32 [w_rows][taps * 3 * C] = per tap [hi | hi | lo].  force_bn: 0 = auto, else 32/64/128/256.                         */
+ * W fp32 [w_rows][taps * 3 * C] = per tap [hi | hi | lo].  force_bn: 0 = auto, else 32/64/128/256 (tf32: 32/64/128; it has
+ * no TMA-store epilogue).                                                                                                 */
 int prisma_debug_gemm_ep(int device, const void* A, long long a_rows, int a_cols, int a_pitch, const void* W, int w_rows,
                          int M, int N, int taps, const int* tap_off, int force_bn, int tf32, int c_half,
                          const prisma_debug_epilogue* ep);

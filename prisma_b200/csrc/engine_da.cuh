@@ -110,7 +110,6 @@ class DepthEngine {
   size_t slot_frames = 0, slot_bytes_frame = 0;
   bool slot_has_pred = false;
   cudaGraphExec_t graph_exec = nullptr;
-  bool use_graph = true;
   bool finalized = false;
   std::map<std::string, HostTensor> host;
   std::vector<void*> allocs, plan_allocs;

@@ -66,9 +66,6 @@ int RaftEngine::init(int dev) {
   num_sms = prop.multiProcessorCount;
   device_mem = prop.totalGlobalMem;
   PRISMA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  const char* ng = getenv("PRISMA_NO_GRAPH");
-  use_graph = !(ng && ng[0] == '1');
-  if (const char* np = getenv("PRISMA_RAFT_PAIRS")) stream_pairs = std::min(std::max(atoi(np), 1), 4);
   return 0;
 }
 
@@ -469,8 +466,8 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
       add("reuse_prev", [=](cudaStream_t s) {
         const size_t n = (size_t)c->rows_pad * c->C * sizeof(__half);
         PRISMA_CUDA_OK(cudaMemcpyAsync(c->feat, c->feat + (size_t)NP * c->rows_pad * c->C, n, cudaMemcpyDeviceToDevice, s));
-        const size_t pn = (size_t)c->rows123_pad * c->C * c->pw * sizeof(__half);
-        PRISMA_CUDA_OK(cudaMemcpyAsync(c->pool123, c->pool123 + (size_t)NP * c->rows123_pad * c->C * c->pw, pn, cudaMemcpyDeviceToDevice, s));
+        const size_t pn = (size_t)c->rows123_pad * c->C * sizeof(__half);
+        PRISMA_CUDA_OK(cudaMemcpyAsync(c->pool123, c->pool123 + (size_t)NP * c->rows123_pad * c->C, pn, cudaMemcpyDeviceToDevice, s));
         PRISMA_CUDA_OK(cudaMemcpyAsync(cn, reinterpret_cast<const char*>(cn) + NP * cn_n, cn_n, cudaMemcpyDeviceToDevice, s));
         PRISMA_CUDA_OK(cudaMemcpyAsync(rsz, rsz + NP * rbytes, rbytes, cudaMemcpyDeviceToDevice, s));
         return 0;
@@ -540,16 +537,13 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
   PRISMA_TRY(new_map(&f1, B, H8, W8, 128, 2));
   __half* f1_cols = nullptr;
   PRISMA_TRY(r_alloc(plan_allocs, &f1_cols, (size_t)B * H8 * W8 * 256));
-  float *zr_f = nullptr, *q_f = nullptr;  // gates in fp32, padded-row layout of the pad-2 maps
-  static const bool fuse_gru = [] { const char* e = getenv("PRISMA_RAFT_FUSE_GRU"); return !(e && e[0] == '0'); }();
+  float* zr_f = nullptr;  // gates in fp32, padded-row layout of the pad-2 maps
   PRISMA_TRY(r_alloc(plan_allocs, &zr_f, (size_t)hx.rows() * 256));
-  PRISMA_TRY(r_alloc(plan_allocs, &q_f, (size_t)hx.rows() * 128));
   PRISMA_TRY(new_map(&fh, B, H8, W8, 256, 2));
   float* fh2_u = nullptr;
   PRISMA_TRY(r_alloc(plan_allocs, &fh2_u, (size_t)hx.rows() * 32));
   PRISMA_TRY(new_map(&mk, B, H8, W8, 256, 2));
   PRISMA_TRY(r_alloc(plan_allocs, &b.mask, (size_t)hx.rows() * 576));
-  const long long rows = hx.rows();
   for (int it = 0; it < iters; ++it) {
     {
       FlowCorr* c = corr; const float* c1p = b.coords1; __half* dst = corrf.p; const int wp = corrf.Wp(), ir = (int)corrf.img_rows();
@@ -583,24 +577,13 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
       add("flow_cols", [=](cudaStream_t s) { return raft_flow_cols(c0, c1p, B, h8, w8, 2, ir8, hxp, rhp, s); });
     }
     for (int pass = 0; pass < 2; ++pass) {  // SepConvGRU horizontal then vertical (update.py:45-60)
-      if (fuse_gru) {
-        // gate arithmetic in the conv epilogues: r * h -> the q conv's operand; h' = (1 - z) h + z q -> fp32 master + operand copy
-        { GemmEpilogue ep; ep.act = 3; ep.out_f32 = zr_f; ep.out_f32_ld = 256;
-          ep.gru = 1; ep.gru_h = b.h_master; ep.gru_rh = rhx.p; ep.gru_rh_ld = 384;
-          PRISMA_TRY(add_conv("gru_zr", hx, 0, w.zr[pass], ep, 1)); }
-        { GemmEpilogue ep; ep.act = 4; ep.out_f32 = b.h_master; ep.out_f32_ld = 128; ep.out_f16 = hx.p; ep.out_f16_ld = 384;
-          ep.gru = 2; ep.gru_h = b.h_master; ep.gru_z = zr_f;
-          PRISMA_TRY(add_conv("gru_q", rhx, 0, w.q[pass], ep, 1)); }
-      } else {
-        { GemmEpilogue ep; ep.act = 3; ep.out_f32 = zr_f; ep.out_f32_ld = 256;
-          PRISMA_TRY(add_conv("gru_zr", hx, 0, w.zr[pass], ep, 1)); }
-        { const float* z = zr_f; const float* hm = b.h_master; __half* rhp = rhx.p;
-          add("gru_rh", [=](cudaStream_t s) { return raft_gru_rh(z, hm, rhp, rows, s); }); }
-        { GemmEpilogue ep; ep.act = 4; ep.out_f32 = q_f; ep.out_f32_ld = 128;
-          PRISMA_TRY(add_conv("gru_q", rhx, 0, w.q[pass], ep, 1)); }
-        { const float* z = zr_f; const float* qq = q_f; float* hm = b.h_master; __half* hxp = hx.p;
-          add("gru_update", [=](cudaStream_t s) { return raft_gru_update(z, qq, hm, hxp, rows, s); }); }
-      }
+      // gate arithmetic in the conv epilogues: r * h -> the q conv's operand; h' = (1 - z) h + z q -> fp32 master + operand copy
+      { GemmEpilogue ep; ep.act = 3; ep.out_f32 = zr_f; ep.out_f32_ld = 256;
+        ep.gru = 1; ep.gru_h = b.h_master; ep.gru_rh = rhx.p; ep.gru_rh_ld = 384;
+        PRISMA_TRY(add_conv("gru_zr", hx, 0, w.zr[pass], ep, 1)); }
+      { GemmEpilogue ep; ep.act = 4; ep.out_f32 = b.h_master; ep.out_f32_ld = 128; ep.out_f16 = hx.p; ep.out_f16_ld = 384;
+        ep.gru = 2; ep.gru_h = b.h_master; ep.gru_z = zr_f;
+        PRISMA_TRY(add_conv("gru_q", rhx, 0, w.q[pass], ep, 1)); }
     }
     { GemmEpilogue ep; ep.act = 2; ep.out_f16 = fh.p; ep.out_f16_ld = 256;            // flow head
       ConvW cw = w.fh1;
@@ -648,19 +631,17 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
   taps["coords1"] = {b.coords1, B * 2, P, 1, 0};
   PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
   plan_H = H; plan_W = W; plan_scale = scale;
-  if (use_graph) {
-    for (int which = 1; which <= 2; ++which) {
-      PRISMA_TRY(run_direct(stream, which));  // warm: per-kernel attributes are set outside the capture
-      PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
-      cudaGraph_t graph = nullptr;
-      PRISMA_CUDA_OK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-      int r = run_direct(stream, which);
-      cudaError_t e = cudaStreamEndCapture(stream, &graph);
-      if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
-      PRISMA_CUDA_OK(e);
-      PRISMA_CUDA_OK(cudaGraphInstantiate(which == 1 ? &graph_exec : &graph_cached, graph, 0));
-      cudaGraphDestroy(graph);
-    }
+  for (int which = 1; which <= 2; ++which) {
+    PRISMA_TRY(run_direct(stream, which));  // warm: per-kernel attributes are set outside the capture
+    PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
+    cudaGraph_t graph = nullptr;
+    PRISMA_CUDA_OK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
+    int r = run_direct(stream, which);
+    cudaError_t e = cudaStreamEndCapture(stream, &graph);
+    if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
+    PRISMA_CUDA_OK(e);
+    PRISMA_CUDA_OK(cudaGraphInstantiate(which == 1 ? &graph_exec : &graph_cached, graph, 0));
+    cudaGraphDestroy(graph);
   }
   return 0;
 }
@@ -686,26 +667,7 @@ int RaftEngine::infer(const uint8_t* prev, const uint8_t* curr, int H, int W, do
   PRISMA_CUDA_OK(cudaMemcpyAsync(b.img + fb, curr, fb, cudaMemcpyHostToDevice, stream));
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (ms_out) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, stream); }
-  if (getenv("PRISMA_RAFT_PROFILE")) {  // per-step CUDA-event times, aggregated by step name (diagnostics)
-    std::vector<cudaEvent_t> ev(steps.size() + 1);
-    for (auto& e : ev) cudaEventCreate(&e);
-    cudaEventRecord(ev[0], stream);
-    for (size_t i = 0; i < steps.size(); ++i) { if (steps[i].group & which) PRISMA_TRY(steps[i].fn(stream)); cudaEventRecord(ev[i + 1], stream); }
-    PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
-    std::map<std::string, std::pair<int, float>> agg;
-    float tot = 0;
-    for (size_t i = 0; i < steps.size(); ++i) {
-      float t = 0;
-      cudaEventElapsedTime(&t, ev[i], ev[i + 1]);
-      agg[steps[i].name].first++; agg[steps[i].name].second += t; tot += t;
-    }
-    for (auto& e : ev) cudaEventDestroy(e);
-    std::vector<std::pair<float, std::string>> v;
-    for (auto& kv : agg) v.push_back({kv.second.second, kv.first + " x" + std::to_string(kv.second.first)});
-    std::sort(v.rbegin(), v.rend());
-    printf("RAFT step profile (%.3f ms total, ungraphed):\n", tot);
-    for (auto& x : v) printf("  %8.3f ms  %5.1f %%  %s\n", x.first, 100.f * x.first / tot, x.second.c_str());
-  } else if (graph_exec) PRISMA_CUDA_OK(cudaGraphLaunch(which == 1 ? graph_exec : graph_cached, stream));
+  if (graph_exec) PRISMA_CUDA_OK(cudaGraphLaunch(which == 1 ? graph_exec : graph_cached, stream));
   else PRISMA_TRY(run_direct(stream, which));
   if (ms_out) cudaEventRecord(e1, stream);
   const size_t n = (size_t)Hs * Ws;

@@ -53,9 +53,9 @@ class RaftEngine {
   double flops = 0, flops_conv = 0, flops_conv_video = 0;  // full pass total; conv GEMMs of the full / video pass
   int profile(int H, int W, double scale, int iters, float* out8);
   bool has_cache() const { return cache_valid; }
-  // Frame pairs per pass of the clip path (infer_stream / time_resident / profile / work_detail): 1..4, default 4
-  // (PRISMA_RAFT_PAIRS overrides), see build_plan; clip_pairs() lowers it for frames whose pyramids would not fit.  The pair call infer() always plans one pair per pass; switching
-  // between the two paths rebuilds the plan.
+  // Frame pairs per pass of the clip path (infer_stream / time_resident / profile / work_detail): 1..4, default 4, see
+  // build_plan; clip_pairs() lowers it for frames whose pyramids would not fit.  The pair call infer() always plans one pair
+  // per pass; switching between the two paths rebuilds the plan.
   int set_pairs_per_pass(int np);
   int pairs_per_pass() const { return stream_pairs; }
   int use_pairs(int np);  // select the plan variant for the next build_plan
@@ -82,7 +82,7 @@ class RaftEngine {
   cudaGraphExec_t graph_exec = nullptr, graph_cached = nullptr;
   int cur_mask = 3;          // steps carry a mask (Step::group): bit 0 = full pass, bit 1 = video pass
   bool cache_valid = false;  // slot NP of the feature buffers holds the last frame of the previous pass
-  bool use_graph = true, finalized = false;
+  bool finalized = false;
   std::map<std::string, HostTensor> host;
   std::vector<void*> allocs, plan_allocs;
   RaftWeights w;

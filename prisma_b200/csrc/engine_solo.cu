@@ -50,8 +50,6 @@ int SoloEngine::init(const std::string& vin, int dev) {
   exact_head = true;  // "<variant>-fast": the single-pass fp16 head of round 1 (not mask-id faithful, ~40 % faster per frame)
   if (v.size() > 5 && v.substr(v.size() - 5) == "-fast") { exact_head = false; v = v.substr(0, v.size() - 5); }
   if (v.size() > 6 && v.substr(v.size() - 6) == "-exact") { exact_backbone = true; v = v.substr(0, v.size() - 6); }
-  if (const char* e = getenv("PRISMA_SOLO_HEAD")) exact_head = std::string(e) != "fast";
-  if (const char* e = getenv("PRISMA_SOLO_BACKBONE")) exact_backbone = std::string(e) == "exact";
   if (!exact_head) exact_backbone = false;  // the fp32-class backbone feeds the fp32-class head
   variant = v;
   if (v == "r101") { const int l[4] = {3, 4, 23, 3}; std::copy(l, l + 4, layers); scale_long = 1333; scale_short = 800; }
@@ -69,8 +67,6 @@ int SoloEngine::init(const std::string& vin, int dev) {
   PRISMA_CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   PRISMA_CUDA_OK(cudaEventCreate(&ev0));
   PRISMA_CUDA_OK(cudaEventCreate(&ev1));
-  const char* ng = getenv("PRISMA_NO_GRAPH");
-  use_graph = !(ng && ng[0] == '1');
   return 0;
 }
 
@@ -307,9 +303,7 @@ int SoloEngine::build_plan(int H, int W) {
   d_inst = nullptr;
   net_shape(H, W, &nh, &nw, &hp, &wp);
   const int zero_off[1] = {0};
-  const char* cur_tag = "pre";
-  step_tag.clear();
-  auto push_step = [&](std::function<int(cudaStream_t)> fn) { steps.push_back(std::move(fn)); step_tag.push_back(cur_tag); };
+  auto push_step = [&](std::function<int(cudaStream_t)> fn) { steps.push_back(std::move(fn)); };
 
   auto new_map = [&](SMap* mm, int h, int w, int c) -> int {
     mm->H = h; mm->W = w; mm->C = c;
@@ -360,7 +354,6 @@ int SoloEngine::build_plan(int H, int W) {
     const int nh_ = nh, nw_ = nw, hp_ = hp, wp_ = wp;
     push_step([=](cudaStream_t s) { return solo_preprocess(img, H, W, nh_, nw_, hp_, wp_, net, rs, s); });
   }
-  cur_tag = "backbone";
   SMap P[5];
   float* P_dense[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // exact backbone: FPN levels as dense fp32 [H*W][256]
   if (exact_backbone) {
@@ -434,7 +427,6 @@ int SoloEngine::build_plan(int H, int W) {
       }
       CX[li] = xs;
     }
-    cur_tag = "fpn";
     float* Ld[4];
     XMap LX[4];
     for (int i = 0; i < 4; ++i) {
@@ -502,7 +494,6 @@ int SoloEngine::build_plan(int H, int W) {
       }
       C[li] = x;
     }
-    cur_tag = "fpn";
     // ---- FPN
     SMap L[4];
     for (int i = 0; i < 4; ++i) {
@@ -540,7 +531,6 @@ int SoloEngine::build_plan(int H, int W) {
   __half* mfeat = nullptr;   // fast head: dense [HW][256] fp16, the "weight" of the dynamic-conv GEMM
   float* mfeat3 = nullptr;   // exact head: dense [HW][3 * 256] fp32 = [hi | hi | lo]
   if (!exact_head) {
-  cur_tag = "mask_feature_head";
   // ---- mask feature head (solov2_head.py:133-150)
   SMap acc;
   PRISMA_TRY(new_map(&acc, fh, fw, 128));
@@ -570,7 +560,6 @@ int SoloEngine::build_plan(int H, int W) {
   PRISMA_TRY(gnconv(acc, 128, mf_pred, nullptr, mfeat));
   taps["mask_feats"] = {mfeat, 2, HW, 256, 0};
 
-  cur_tag = "towers";
   // ---- head towers (solov2_head.py:253-292, resize_feats solo_head.py:133-153)
   SMap R0, R4;
   PRISMA_TRY(new_map(&R0, P[1].H, P[1].W, 256));
@@ -623,7 +612,6 @@ int SoloEngine::build_plan(int H, int W) {
   { GemmEpilogue ep; ep.bias = conv_cls.b; PRISMA_TRY(conv_t(cb, 512, conv_cls, ep, cls_all)); }
   } else {
   // ================================================================ fp32-class head (solo_exact.cu, gemm_prepare_tf32x3)
-  cur_tag = "mask_feature_head";
   auto new_xmap = [&](XMap* mm, int h, int w, int c) -> int {
     mm->H = h; mm->W = w; mm->C = c;
     return s_alloc(plan_allocs, &mm->p, (size_t)mm->rows() * 2 * c);
@@ -692,7 +680,6 @@ int SoloEngine::build_plan(int H, int W) {
   PRISMA_TRY(gnconv_x(accx, 128, mf_pred3, nullptr, mfeat3));
   taps["mask_feats"] = {mfeat3, 6, HW, 256, 0};
 
-  cur_tag = "towers";
   XMap R0x, R4x;
   PRISMA_TRY(new_xmap(&R0x, P[1].H, P[1].W, 256));
   PRISMA_TRY(new_xmap(&R4x, P[3].H, P[3].W, 256));
@@ -750,7 +737,6 @@ int SoloEngine::build_plan(int H, int W) {
     taps["kernel" + std::to_string(l)] = {ker_out[l], 5, num_grids[l], 256, F};
   }
 
-  cur_tag = "decode";
   // ---- decode (solov2_head.py:582-766)
   SoloCand *cand_raw = nullptr, *cand = nullptr;
   PRISMA_TRY(s_alloc(plan_allocs, &cand_raw, (size_t)SOLO_CAP));
@@ -843,19 +829,17 @@ int SoloEngine::build_plan(int H, int W) {
   PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
   plan_H = H; plan_W = W;
   if (graph_exec) { cudaGraphExecDestroy(graph_exec); graph_exec = nullptr; }
-  if (use_graph) {
-    PRISMA_TRY(run(stream));  // warm: per-kernel attributes are set outside the capture
-    PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
-    cudaGraph_t graph = nullptr;
-    PRISMA_CUDA_OK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    int r = 0;
-    for (auto& st : steps) { r = st(stream); if (r != 0) break; }
-    cudaError_t e = cudaStreamEndCapture(stream, &graph);
-    if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
-    PRISMA_CUDA_OK(e);
-    PRISMA_CUDA_OK(cudaGraphInstantiate(&graph_exec, graph, 0));
-    cudaGraphDestroy(graph);
-  }
+  PRISMA_TRY(run(stream));  // warm: per-kernel attributes are set outside the capture
+  PRISMA_CUDA_OK(cudaStreamSynchronize(stream));
+  cudaGraph_t graph = nullptr;
+  PRISMA_CUDA_OK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
+  int r = 0;
+  for (auto& st : steps) { r = st(stream); if (r != 0) break; }
+  cudaError_t e = cudaStreamEndCapture(stream, &graph);
+  if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
+  PRISMA_CUDA_OK(e);
+  PRISMA_CUDA_OK(cudaGraphInstantiate(&graph_exec, graph, 0));
+  cudaGraphDestroy(graph);
   return 0;
 }
 
@@ -873,21 +857,6 @@ int SoloEngine::infer(const uint8_t* rgb, int H, int W, float confidence, uint8_
   PRISMA_TRY(build_plan(H, W));
   if (inst_masks_out && !d_inst) PRISMA_TRY(s_alloc(plan_allocs, &d_inst, (size_t)SOLO_MAX * H * W));
   PRISMA_CUDA_OK(cudaMemcpyAsync(d_img, rgb, (size_t)H * W * 3, cudaMemcpyHostToDevice, stream));
-  if (getenv("PRISMA_SOLO_PROFILE")) {  // per-stage device times of one ungraphed pass (stderr)
-    std::map<std::string, float> acc;
-    cudaEvent_t a, b2;
-    cudaEventCreate(&a); cudaEventCreate(&b2);
-    for (size_t i = 0; i < steps.size(); ++i) {
-      cudaEventRecord(a, stream);
-      PRISMA_TRY(steps[i](stream));
-      cudaEventRecord(b2, stream);
-      cudaEventSynchronize(b2);
-      float ms = 0; cudaEventElapsedTime(&ms, a, b2);
-      acc[step_tag[i]] += ms;
-    }
-    cudaEventDestroy(a); cudaEventDestroy(b2);
-    for (auto& kv : acc) fprintf(stderr, "[solo-profile] %-20s %8.3f ms\n", kv.first.c_str(), kv.second);
-  }
   PRISMA_CUDA_OK(cudaEventRecord(ev0, stream));
   PRISMA_TRY(run(stream));
   if (exact_head)

@@ -56,11 +56,10 @@ class SoloEngine {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
-  bool use_graph = true, finalized = false;
+  bool finalized = false;
   std::map<std::string, HostTensor> host;
   std::vector<void*> allocs, plan_allocs;
   std::vector<std::function<int(cudaStream_t)>> steps;
-  std::vector<const char*> step_tag;  // stage of each step (PRISMA_SOLO_PROFILE)
   std::map<std::string, SoloTap> taps;
   // weights
   SoloConvW stem;

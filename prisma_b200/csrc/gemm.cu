@@ -11,14 +11,6 @@ namespace prisma {
 NvtxRange::NvtxRange(const char* name) { nvtxRangePushA(name); }
 NvtxRange::~NvtxRange() { nvtxRangePop(); }
 
-// Programmatic dependent launch is OFF unless PRISMA_PDL=1: the ~330 kernels of a RAFT pass are already back to back inside
-// a CUDA graph, and tests/test_raft_gpu.py has seen a wrong max displacement under it (an ordering it must not change).
-// Kept only as an experiment switch.
-bool pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("PRISMA_PDL"); return e && e[0] == '1'; }();
-  return on;
-}
-
 int device_sm_count() {
   static std::atomic<int> cache[64] = {};  // engines on several threads (mask lanes) query it concurrently
   int dev = 0;
@@ -138,17 +130,13 @@ int gemm_prepare_tf32x3(GemmLaunch* out, const float* A_split, long long a_rows,
                         int M, int N, int taps, const int* tap_off, const GemmEpilogue& ep, int num_sms, int force_bn) {
   PRISMA_CHECK(taps * 3 <= GEMM_MAX_TAPS, "gemm(tf32x3): too many taps");
   PRISMA_CHECK(C % 32 == 0 && C_half % 32 == 0 && C <= C_half, "gemm(tf32x3): channel counts must be multiples of 32");
+  // external accumulation keeps 64 running-sum registers per thread: 128-wide tiles at most
+  PRISMA_CHECK(force_bn != 256, "gemm(tf32x3): external accumulation needs BLOCK_N <= 128");
   int off[GEMM_MAX_TAPS], acol[GEMM_MAX_TAPS];
   for (int t = 0; t < taps; ++t)
     for (int p = 0; p < 3; ++p) { off[t * 3 + p] = tap_off[t]; acol[t * 3 + p] = p == 1 ? C_half : 0; }
-  // external accumulation (GemmArgs::acc_group): 128-wide tiles at most (the running sums are 64 registers per thread).
-  // PRISMA_TF32_ACC_GROUP=0 keeps the whole K inside one wgmma chain (the biased, cheaper variant).
-  static const int acc_group = [] { const char* e = getenv("PRISMA_TF32_ACC_GROUP"); return e ? atoi(e) : 4; }();
-  if (acc_group > 0 && force_bn == 0) force_bn = N > 64 ? 128 : (N > 32 ? 64 : 32);
-  PRISMA_TRY(gemm_prepare_impl(out, A_split, a_rows, C, 2 * C_half, W3, w_rows, M, N, taps * 3, off, acol, ep, num_sms, force_bn, true));
-  out->args.acc_group = acc_group > 0 ? acc_group : 1;
-  out->xacc = acc_group > 0 && out->bn <= 128;
-  return 0;
+  if (force_bn == 0) force_bn = N > 64 ? 128 : (N > 32 ? 64 : 32);
+  return gemm_prepare_impl(out, A_split, a_rows, C, 2 * C_half, W3, w_rows, M, N, taps * 3, off, acol, ep, num_sms, force_bn, true);
 }
 
 static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, int a_cols, int a_pitch, const void* W,
@@ -157,18 +145,13 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
   PRISMA_CHECK(taps >= 1 && taps <= GEMM_MAX_TAPS, "gemm: bad tap count");
   PRISMA_CHECK(N % 4 == 0, "gemm: N must be a multiple of 4");
   PRISMA_CHECK(M >= 1 && a_cols >= 1, "gemm: empty problem");
-  // force_bn: 32 / 64 / 128 / 256.  512, 384 and 640 name the 256 x 256, 256 x 128 and transposed 128 x 256 tiles of the
-  // sm_100 build (CTA pairs, swapped operands); Hopper has no such instructions, so they request the 256- / 128-wide tiles.
-  int bn = force_bn ? force_bn : gemm_pick_bn(M, N, num_sms);
-  if (bn == 512) bn = 256;
-  else if (bn == 384 || bn == 640) bn = 128;
+  const int bn = force_bn ? force_bn : gemm_pick_bn(M, N, num_sms);  // force_bn: 32 / 64 / 128 / 256
   GemmEpilogue ep = ep_in;
   // the TMA-store epilogue exists for 128- and 256-wide tiles; a problem the tile choice gives narrower tiles keeps the
   // register epilogue (same results: the TMA path is an optimisation of the same arithmetic)
   if (ep.tma_store && (bn == 32 || bn == 64) && !tf32) ep.tma_store = false;
+  PRISMA_CHECK(!(ep.tma_store && tf32), "gemm(tf32x3): the TMA-store epilogue exists for the fp16 path only");
   out->tf32 = tf32;
-  out->xacc = false;
-  out->args.acc_group = 1;
   const int bke = tf32 ? 32 : 64;  // elements per 128-byte K block
   PRISMA_CHECK(bn == 32 || bn == 64 || bn == 128 || bn == 256, "gemm: unsupported BLOCK_N");
   // preconditions of the fused epilogues (without them the kernel writes wrong cells without any error)
@@ -187,10 +170,7 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
   out->args.N = N;
   out->args.taps = taps;
   out->args.kchunks = kchunks;
-  {
-    static const char* r = getenv("PRISMA_GEMM_RASTER");  // "m" / "n": force (experiments)
-    out->args.raster_n = r ? (r[0] == 'n') : (M >= N);
-  }
+  out->args.raster_n = M >= N;
   for (int t = 0; t < GEMM_MAX_TAPS; ++t) {
     out->args.tap_off[t] = t < taps ? tap_off[t] : 0;
     out->args.tap_acol[t] = (t < taps && tap_acol) ? tap_acol[t] : 0;
@@ -231,38 +211,27 @@ static int gemm_prepare_impl(GemmLaunch* out, const void* A, long long a_rows, i
   return 0;
 }
 
-template <int BN, bool TMAST = false, bool TF32 = false, bool XACC = false>
+template <int BN, bool TMAST = false, bool TF32 = false>
 static int launch_bn(const GemmLaunch& g, cudaStream_t stream) {
   static bool attr_set = false;  // per-process, per-instantiation
   using Cfg = GemmCfg<BN, TMAST>;
   if (!attr_set) {
-    PRISMA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, TMAST, TF32, XACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    PRISMA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, TMAST, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
-  PRISMA_CUDA_OK(pdl_launch(gemm_tc_kernel<BN, TMAST, TF32, XACC>, dim3(g.grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream,
-                            g.tmA, g.tmB, g.tmD, g.args));
+  gemm_tc_kernel<BN, TMAST, TF32><<<g.grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(g.tmA, g.tmB, g.tmD, g.args);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
 int gemm_run(const GemmLaunch& g, cudaStream_t stream) {
-  if (g.tf32 && g.xacc) {
-    switch (g.bn) {
-      case 128: return launch_bn<128, false, true, true>(g, stream);
-      case 64: return launch_bn<64, false, true, true>(g, stream);
-      case 32: return launch_bn<32, false, true, true>(g, stream);
-    }
-    set_last_error("gemm_run: external accumulation needs BLOCK_N <= 128");
-    return -1;
-  }
   if (g.tf32) {
     switch (g.bn) {
-      case 256: return launch_bn<256, false, true>(g, stream);
       case 128: return launch_bn<128, false, true>(g, stream);
       case 64: return launch_bn<64, false, true>(g, stream);
       case 32: return launch_bn<32, false, true>(g, stream);
     }
-    set_last_error("gemm_run: unsupported BLOCK_N (tf32)");
+    set_last_error("gemm_run: external accumulation needs BLOCK_N <= 128");
     return -1;
   }
   if (g.tma_store) {

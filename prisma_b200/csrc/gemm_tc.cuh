@@ -28,6 +28,9 @@ constexpr int GEMM_BK = 64;
 constexpr int GEMM_THREADS = 384;                           // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int GEMM_SMEM_MAX = 232448;                       // 227 KB of dynamic shared memory per CTA
 constexpr int GEMM_MAX_TAPS = 49;
+// 3xTF32 path: K blocks accumulated inside one wgmma chain before the partial sum is added to the running fp32 sums with
+// round-to-nearest FADDs (external accumulation, see gemm_tc_kernel)
+constexpr int GEMM_TF32_ACC_GROUP = 4;
 
 enum RowMap : int {
   ROW_LINEAR = 0,   // dst row = m                                   (valid: m < M)
@@ -115,8 +118,6 @@ struct GemmArgs {
   int tap_off[GEMM_MAX_TAPS];
   int tap_acol[GEMM_MAX_TAPS];  // first A column (elements) of each tap's K slab: 0 for plain convs; the 3xTF32 path walks
                                 // [hi | lo] activation halves: (hi, W_hi), (lo, W_hi), (hi, W_lo)
-  int acc_group;  // XACC kernels: K blocks accumulated inside one wgmma chain before the partial sum is added to the running
-                  // fp32 sums with round-to-nearest FADDs (see gemm_prepare_tf32x3)
   int raster_n;  // 1: consecutive tiles walk N first (the CTAs of a wave share few A row panels and all of W: A is read
                  // from HBM once when M >> N); 0: M first
   GemmEpilogue ep;
@@ -330,7 +331,7 @@ __device__ __forceinline__ void stage_fragment(const float* d, int cb, uint32_t 
   }
 }
 
-template <int BN, bool TMAST, bool TF32, bool XACC>
+template <int BN, bool TMAST, bool TF32>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmD, const __grid_constant__ GemmArgs args) {
@@ -346,7 +347,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
 
-  pdl_launch_dependents();  // the next kernel may be scheduled behind this one (see common.cuh)
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
@@ -358,9 +358,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     fence_mbar_init();
   }
   __syncthreads();
-  pdl_wait();  // barriers and descriptors are set up; from here on the predecessor's results are read
 
-  // *m_dev is written by the previous kernel (the SOLOv2 candidate count), so it is read only after the wait
+  // *m_dev (the SOLOv2 candidate count) is written by an earlier kernel of the stream, which has completed by launch order
   const int M_run = args.ep.m_dev ? min(args.M, (*args.ep.m_dev + GEMM_BM - 1) / GEMM_BM * GEMM_BM) : args.M;  // see GemmEpilogue::m_dev
   const int tiles_m = (M_run + GEMM_BM - 1) / GEMM_BM;
   const int tiles_n = (args.N + BN - 1) / BN;
@@ -404,14 +403,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int cg = lane & 7;     // coalesced phase: which 4-column group of the 32-column chunk
     const int rsub = lane >> 3;  // coalesced phase: row offset inside a 4-row step
     float acc[BN / 2];
-    float run[XACC ? BN / 2 : 1];
+    float run[TF32 ? BN / 2 : 1];
     int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int tm, tn;
       tile_mn(tile, &tm, &tn);
       const int m0 = tm * GEMM_BM, n0 = tn * BN;
       // ---- mainloop
-      if (XACC) {
+      if (TF32) {
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) run[i] = 0.f;
       }
@@ -420,10 +419,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         mbar_wait(&full[stage], phase);
         const uint64_t adesc = make_wgmma_desc(smem_u32(sA + stage * Cfg::A_BYTES + wg * 64 * 128));
         const uint64_t bdesc = make_wgmma_desc(smem_u32(sB + stage * Cfg::B_BYTES));
-        // External accumulation (XACC): the tensor core adds into its fp32 accumulator by TRUNCATING the aligned addend, a
-        // bias that grows with the length of the chain.  Here a chain is only `acc_group` K blocks long; every finished
-        // partial sum is added to register-resident running sums with round-to-nearest FADDs.
-        const bool first = XACC ? (kb % args.acc_group) == 0 : kb == 0;
+        // External accumulation (3xTF32): the tensor core adds into its fp32 accumulator by TRUNCATING the aligned addend, a
+        // bias that grows with the length of the chain.  Here a chain is only GEMM_TF32_ACC_GROUP K blocks long; every
+        // finished partial sum is added to register-resident running sums with round-to-nearest FADDs.
+        const bool first = TF32 ? (kb % GEMM_TF32_ACC_GROUP) == 0 : kb == 0;
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GEMM_BK / 16; ++k) {
@@ -433,9 +432,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         wgmma_commit();
         // one wgmma group stays in flight while the next stage is waited for: a stage is released when the group that
-        // read it has retired, one K block later; the chain is drained at the end of a tile (and at the end of an XACC
-        // group, whose partial sum is read here)
-        if (XACC && (kb % args.acc_group) == args.acc_group - 1 && kb != num_kb - 1) {
+        // read it has retired, one K block later; the chain is drained at the end of a tile (and at the end of a 3xTF32
+        // accumulation group, whose partial sum is read here)
+        if (TF32 && (kb % GEMM_TF32_ACC_GROUP) == GEMM_TF32_ACC_GROUP - 1 && kb != num_kb - 1) {
           wgmma_wait<0>();
           if ((threadIdx.x & 127) == 0) {
             if (prev_stage >= 0) mbar_arrive(&empty[prev_stage]);
@@ -453,11 +452,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       wgmma_wait<0>();
       if ((threadIdx.x & 127) == 0 && prev_stage >= 0) mbar_arrive(&empty[prev_stage]);
-      if (XACC) {
+      if (TF32) {
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) run[i] += acc[i];
       }
-      const float* fin = XACC ? run : acc;
+      const float* fin = TF32 ? run : acc;
 
       if (TMAST) {
         // ---- TMA-store path: scaled (+ bias, LayerScale / activation) values straight into the swizzled boxes of the warp
@@ -602,9 +601,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
           for (int rr = 0; rr < 8; ++rr)
             drs[rr] = ib8[rr] + (ty8[rr] * ep.shuf_s + sdy + out_ld) * ep.out_wp + tx8[rr] * ep.shuf_s + sdx + out_ld;
-          epilogue_rows8<!TF32 && !XACC>(ep, v, drs, ncol_ok ? okrows : 0u, bias4, gamma4, col);
+          epilogue_rows8<!TF32>(ep, v, drs, ncol_ok ? okrows : 0u, bias4, gamma4, col);
         } else {
-          epilogue_rows8<!TF32 && !XACC>(ep, v, dr8, ncol_ok ? okrows : 0u, bias4, gamma4, col);
+          epilogue_rows8<!TF32>(ep, v, dr8, ncol_ok ? okrows : 0u, bias4, gamma4, col);
         }
         if (ep.stat_part != nullptr) {
           float4 sm = make_float4(0.f, 0.f, 0.f, 0.f), sq = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -640,7 +639,6 @@ struct GemmLaunch {
   CUtensorMap tmA, tmB;
   CUtensorMap tmD;             // dense output, 32-row boxes (TMA-store epilogue only)
   bool tma_store = false;
-  bool xacc = false;           // external fp32 accumulation (tf32x3 only): see GemmArgs::acc_group
   bool tf32 = false;           // tf32 operands (fp32 containers): the 3xTF32 "fp32-class" path of the mask band
   GemmArgs args;
   int bn = 128;
@@ -655,7 +653,8 @@ int gemm_prepare(GemmLaunch* out, const __half* A, long long a_rows, int a_cols,
 // 3xTF32: A = fp32 [a_rows][2 * C_half] holding [hi | lo] halves (hi = the top 19 bits of the value, lo = value - hi) of
 // which the first C channels enter the product, W = fp32 [w_rows][taps * 3 * C] holding per tap [W_hi | W_hi | W_lo];
 // D = sum_t (hi . W_hi + lo . W_hi + hi . W_lo): fp32-class products (the dropped lo . W_lo term is 2^-22 relative), fp32
-// accumulate.  Same epilogues.  C, C_half multiples of 32.
+// accumulate with external accumulation (GEMM_TF32_ACC_GROUP), so tiles are at most 128 wide.  Same epilogues except the
+// TMA store and the ConvGRU gates.  C, C_half multiples of 32.
 int gemm_prepare_tf32x3(GemmLaunch* out, const float* A_split, long long a_rows, int C, int C_half, const float* W3, int w_rows,
                         int M, int N, int taps, const int* tap_off, const GemmEpilogue& ep, int num_sms, int force_bn = 0);
 int gemm_run(const GemmLaunch& g, cudaStream_t stream);

@@ -828,6 +828,9 @@ REFUSED = {
     "gru 1 with N != 256": dict(gru=1, gru_h="other", gru_rh="half", N=128),
     "gru 2 with N != 128": dict(gru=2, gru_h="other", gru_z="other", N=256),
     "gru on the 3xTF32 path": dict(gru=2, gru_h="other", gru_z="other", N=128, tf32=True),
+    "tma_store on the 3xTF32 path": dict(tma_store=1, tf32=True),
+    "force_bn 256 on the 3xTF32 path": dict(tf32=True, bn=256),
+    "force_bn 512": dict(bn=512),
 }
 
 
@@ -839,6 +842,7 @@ def test_refused_configurations(case):
     cfg = dict(REFUSED[case])
     N = cfg.pop("N", 128)
     tf32 = cfg.pop("tf32", False)
+    bn = cfg.pop("bn", 128)
     M, K = 256, 64
     rng = np.random.default_rng(7)
     A = exact_rows(rng, M, K)
@@ -852,9 +856,9 @@ def test_refused_configurations(case):
             fields[k + "_ld"] = 256
     ep = make_ep(**fields)
     if tf32:
-        rc = run(upload_a_tf32(A, K), upload_w_tf32(w), K, M, N, [0], ep, bn=128, tf32=True, c_half=K)
+        rc = run(upload_a_tf32(A, K), upload_w_tf32(w), K, M, N, [0], ep, bn=bn, tf32=True, c_half=K)
     else:
-        rc = run(upload_a16(A, K), upload_w16(w), K, M, N, [0], ep, bn=128)
+        rc = run(upload_a16(A, K), upload_w16(w), K, M, N, [0], ep, bn=bn)
     assert rc < 0, f"{case}: accepted"
     assert "gemm" in _lib().prisma_last_error().decode()
     assert torch.isnan(out).all() and torch.isnan(bufs["half"].float()).all() and torch.isnan(bufs["stats"]).all()

@@ -34,24 +34,24 @@ def _gemm(A, W, bias, act, bn):
     (333, 32, 1152, 2, 32),      # BN=32
     (40000, 256, 128, 0, 0),     # many tiles per CTA (persistent loop, operand ring wrapping across tiles)
     (64, 64, 64, 0, 0),          # smaller than a tile
-    (512, 256, 128, 0, 512),     # force_bn 512 -> 256-wide tiles: four row tiles, one column tile
-    (2443, 3072, 1024, 0, 512),  # 256-wide tiles, ViT-L qkv: ragged M, several tiles per CTA
-    (9772, 1024, 4096, 1, 512),  # 256-wide tiles, 4-frame fc2 shape with gelu (long K: the operand ring wraps many times)
-    (300, 256, 200, 2, 512),     # 256-wide tiles: the last row tile's slabs partly / fully out of range, K tail
-    (37000, 128, 1920, 0, 384),  # force_bn 384 -> 128-wide tiles (the RAFT GRU q conv shape), ragged M
-    (700, 256, 320, 2, 384),     # 128-wide tiles, two column tiles, K tail
+    (512, 256, 128, 0, 256),     # 256-wide tiles: four row tiles, one column tile
+    (2443, 3072, 1024, 0, 256),  # 256-wide tiles, ViT-L qkv: ragged M, several tiles per CTA
+    (9772, 1024, 4096, 1, 256),  # 256-wide tiles, 4-frame fc2 shape with gelu (long K: the operand ring wraps many times)
+    (300, 256, 200, 2, 256),     # 256-wide tiles: the last row tile's slabs partly / fully out of range, K tail
+    (37000, 128, 1920, 0, 128),  # 128-wide tiles (the RAFT GRU q conv shape), ragged M
+    (700, 256, 320, 2, 128),     # 128-wide tiles, two column tiles, K tail
     # auto tile choice (gemm_pick_bn) with a partial last wave
     (29316, 1024, 192, 0, 0),    # ViT-L fc1-like rows, short K
     (26624, 256, 128, 2, 0),     # relu, two 128-wide or one 256-wide column tile
     (39008, 128, 384, 1, 0),     # 305 row tiles on 132 SMs (2.3 waves), gelu
     (20000, 64, 128, 0, 0),      # narrow N: 157 row tiles
-    # force_bn 640 -> 128-wide tiles; N <= 128 shapes with ragged edges
-    (256, 128, 64, 0, 640),      # two row tiles, one k-block
-    (37000, 128, 1920, 0, 640),  # the RAFT GRU q conv shape: ragged M, many tiles per CTA
-    (5000, 96, 576, 2, 640),     # N = 96 (RAFT encoder layer 2): the last 32-column chunk is beyond N; relu
-    (777, 128, 200, 1, 640),     # K tail, gelu, M not a multiple of 32
+    # 128-wide tiles; N <= 128 shapes with ragged edges
+    (256, 128, 64, 0, 128),      # two row tiles, one k-block
+    (37000, 128, 1920, 0, 128),  # the RAFT GRU q conv shape: ragged M, many tiles per CTA
+    (5000, 96, 576, 2, 128),     # N = 96 (RAFT encoder layer 2): the last 32-column chunk is beyond N; relu
+    (777, 128, 200, 1, 128),     # K tail, gelu, M not a multiple of 32
     (151552, 128, 256, 0, 0),    # auto choice, N = 128, 1184 row tiles: many tiles per CTA
-    (4100, 68, 128, 0, 640),     # N % 32 = 4: one 4-column group of the third 32-column chunk valid
+    (4100, 68, 128, 0, 128),     # N % 32 = 4: one 4-column group of the third 32-column chunk valid
 ])
 def test_gemm_matches_fp32_reference(M, N, K, act, bn):
     rng = np.random.default_rng(M * 7 + N * 3 + K)
@@ -71,7 +71,7 @@ def test_gemm_matches_fp32_reference(M, N, K, act, bn):
 
 @pytest.mark.parametrize("M,N,K,bn", [
     (18360, 18360, 256, 0),   # RAFT correlation level 0 at 1080p x 0.75: ragged M and N (N % 32 = 24)
-    (18360, 4592, 512, 0),    # level 1 (hi/lo pooled features: K = 512), N % 32 = 16
+    (18360, 4592, 512, 0),    # level 1 size class with K = 512, N % 32 = 16
     (1000, 264, 256, 128),    # level 3 size class, 128-wide tiles
     (300, 520, 64, 256),      # 256-wide, rows of the last tile out of range
 ])
@@ -91,7 +91,7 @@ def test_gemm_tma_store_epilogue(M, N, K, bn):
 
 @pytest.mark.parametrize("M,N,K,bn", [
     (18360, 18360, 256, 0),   # RAFT correlation level 0 at 1080p x 0.75: ragged M and N (N % 32 = 24)
-    (18360, 4592, 512, 0),    # level 1 (hi/lo pooled features: K = 512), N % 32 = 16
+    (18360, 4592, 512, 0),    # level 1 size class with K = 512, N % 32 = 16
     (1000, 264, 256, 128),    # level 3 size class, 128-wide tiles
     (300, 520, 64, 256),      # 256-wide, rows of the last tile out of range
 ])
@@ -178,9 +178,9 @@ def test_conv_matches_torch(H, W, Cin, Cout, k, relu):
 def test_gemm_tf32x3_is_fp32_class(M, N, K, bn):
     """The 3xTF32 path (tf32 MMAs on [hi | lo] splits of both operands) against the exact product (float64).  The
     products are fp32-class (the dropped lo x lo term is 2^-22).  The tensor core's own fp32 ACCUMULATION truncates the aligned
-    addends instead of rounding them, a bias that grows with K (PRISMA_TF32_ACC_GROUP=0 reproduces it).  The kernel
+    addends instead of rounding them, a bias that grows with K (a single wgmma chain over the whole K reproduces it).  The kernel
     therefore keeps a wgmma chain 4 K-blocks (16 MMAs) long and adds the partial sums in registers with round-to-nearest
-    FADDs (GemmArgs::acc_group): the error is then that of a CUDA-core fp32 GEMM."""
+    FADDs (GEMM_TF32_ACC_GROUP): the error is then that of a CUDA-core fp32 GEMM."""
     rng = np.random.default_rng(M + N + K)
     A = (rng.standard_normal((M, K), dtype=np.float32) * rng.uniform(0.01, 30.0, (M, 1)).astype(np.float32))
     W = (rng.standard_normal((N, K), dtype=np.float32) / np.sqrt(K)).astype(np.float32)
