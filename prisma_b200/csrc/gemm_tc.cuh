@@ -8,15 +8,24 @@
 //                             rows.  Border rows are computed and discarded (waste 2/(W+2)); no im2col buffer, no 4-D
 //                             tensor map; TMA zero-fills out-of-range rows (either sign).
 //
-// Kernel anatomy (persistent, warp-specialised, one CTA per SM, 384 threads):
+// Kernel anatomy (persistent, warp-specialised, one CTA per SM):
 //   warpgroups 0-1 : consumers  (each: wgmma.mma_async M=64 x N=BN x K=16 over its 64 rows of the 128-row tile, fp32
-//                                accumulators in registers; then the epilogue of those rows)
+//                                accumulators in registers)
 //   warpgroup  2   : producer   (one thread: TMA loads of A 128x64 and W BNx64 fp16 tiles, 128B swizzle, STAGES-deep
-//                                mbarrier ring; its registers are handed to the consumers with setmaxnreg)
-// Epilogue: a warp holds 16 accumulator rows; the two warps of a pair (32 consecutive rows) exchange their fragments through
-// their swizzled 32 x 32 fp32 staging buffers, so that each then owns one 32-row x 32-column chunk and applies bias / GELU /
-// ReLU / LayerScale / residuals with coalesced fp32 and/or fp16 stores in the row mapping of the consumer's layout (every
-// global access of a chunk is issued as a batch of 8 independent requests per lane), or stores it with TMA.
+//                                mbarrier ring; its registers are handed to the other roles with setmaxnreg)
+//   warpgroup  3   : epilogue   (fp16 register-epilogue kernels only, 512 threads; see below)
+// Two schedules run the epilogue (GemmCfg::EPI_WG):
+//   * fp16 operands with the register epilogue, BN <= 128 (512 threads): after a tile's mainloop the consumers write their raw
+//     fp32 accumulators into a 128-row x BN-column shared-memory hand-off buffer (swizzled 32 x 32 fp32 boxes, one per
+//     32-row slab and 32-column chunk) and go straight on to the next tile's MMAs.  Epilogue warp w owns slab w: it reads
+//     each chunk of its slab from the buffer, releases the buffer after its last read and then loads residuals / gate
+//     inputs and stores, while the tensor cores run the next tile.
+//   * 3xTF32, the TMA store and 256-wide fp16 tiles keep the consumer-run epilogue (384 threads): a warp holds 16
+//     accumulator rows; the two warps of a pair (32 consecutive rows) exchange their fragments through their swizzled
+//     32 x 32 fp32 staging buffers, so that each then owns one 32-row x 32-column chunk, or stage whole boxes for TMA.
+// Either way a 32-row x 32-column chunk gets bias / GELU / ReLU / LayerScale / residuals with coalesced fp32 and/or fp16 stores
+// in the row mapping of the consumer's layout (epilogue_chunk; every global access of a chunk is issued as a batch of 8
+// independent requests per lane).
 #pragma once
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -25,7 +34,6 @@ namespace prisma {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 384;                           // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int GEMM_SMEM_MAX = 232448;                       // 227 KB of dynamic shared memory per CTA
 constexpr int GEMM_MAX_TAPS = 49;
 // 3xTF32 path: K blocks accumulated inside one wgmma chain before the partial sum is added to the running fp32 sums with
@@ -123,13 +131,32 @@ struct GemmArgs {
   GemmEpilogue ep;
 };
 
-template <int BN, bool TMAST = false>  // TMAST: TMA-store epilogue (double-buffered staging boxes)
+// TMAST: TMA-store epilogue (double-buffered staging boxes); TF32: 3xTF32 operands.  The fp16 register-epilogue kernels up
+// to 128 columns run their epilogue in a warpgroup of its own (EPI_WG) behind a shared-memory hand-off buffer.  A 512-thread
+// CTA leaves ptxas 128 registers per thread in every role (65536 / 512), and a 128 x 256 tile's consumers need 128 for the
+// accumulators alone, so 256-wide tiles keep the 384-thread schedule with the consumer-run epilogue.
+template <int BN, bool TMAST = false, bool TF32 = false>
 struct GemmCfg {
+  static constexpr bool EPI_WG = !TMAST && !TF32 && BN <= 128;
+  static constexpr int THREADS = EPI_WG ? 512 : 384;
+  // setmaxnreg counts of the roles (registers per thread), 2 x consumer + producer (+ epilogue) <= 65536 / 128 = 512:
+  //   EPI_WG (512 threads): consumers 152, producer 40, epilogue 168
+  //   384 threads         : consumers 232, producer 40
+  // ptxas allocates at most 65536 / THREADS registers per thread (128 / 168) in every role; the counts above leave the
+  // surplus with the roles that can use it.  ptxas -v: the EPI_WG kernels use 128 registers without spills; the 384-thread
+  // fp16 BN 256 and 3xTF32 BN 128 kernels spill 176 / 132 bytes
+  // (168 / 132 before the epilogue warpgroup existed).
+  static constexpr int REGS_CONSUMER = EPI_WG ? 152 : 232;
+  static constexpr int REGS_PRODUCER = 40;
+  static constexpr int REGS_EPILOGUE = EPI_WG ? 512 - 2 * REGS_CONSUMER - REGS_PRODUCER : 0;
+  static_assert(2 * REGS_CONSUMER + REGS_PRODUCER + REGS_EPILOGUE <= (EPI_WG ? 512 : 504), "register budget");
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;  // 128 rows x 128 B (64 fp16, or 32 fp32 on the tf32 path)
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STG_WARP = TMAST ? 8192 : 4096;     // per consumer warp: one (two) 32 x 128 B boxes
-  static constexpr int STG_BYTES = 8 * STG_WARP;
+  // EPI_WG: the hand-off buffer, 128 rows x BN fp32 columns as 32 x 32 boxes (box = slab * BN / 32 + chunk);
+  // otherwise the staging boxes of the 8 consumer warps
+  static constexpr int STG_BYTES = EPI_WG ? GEMM_BM * BN * 4 : 8 * STG_WARP;
   static constexpr int FIT = (GEMM_SMEM_MAX - STG_BYTES - 1280) / STAGE_BYTES;  // operand stages that fit beside the staging
   static constexpr int STAGES = FIT > 8 ? 8 : FIT;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
@@ -331,11 +358,158 @@ __device__ __forceinline__ void stage_fragment(const float* d, int cb, uint32_t 
   }
 }
 
+// Row mapping of the 32 output rows of one slab (first row m_slab): lane == row inside the slab for m / valid / the head's
+// pixel, and the 8 rows rr * 4 + lane / 8 this lane stores in the coalesced phase.
+struct SlabRows {
+  int m, valid;
+  int dr8[8], ty8[8], tx8[8], ib8[8];  // destination row; ROW_SHUFFLE: token coordinates and image base row
+  uint32_t okrows;
+};
+
+__device__ __forceinline__ void map_slab_rows(const GemmEpilogue& ep, int M, int m_slab, int lane, SlabRows& s) {
+  const int rsub = lane >> 3;
+  int ty = 0, tx = 0, img_base = 0;
+  const int out_ld = ep.out_lead < 0 ? ep.out_pad : ep.out_lead;  // leading border of the destination map
+  const int m = m_slab + lane;
+  int valid = m < M, drow = m;
+  if (ep.row_map == ROW_PADDED || ep.row_map == ROW_PAD2TOK) {
+    int img = 0, r = m;
+    if (ep.img_rows > 0) { img = m / ep.img_rows; r = m - img * ep.img_rows; }
+    const int y = r / ep.in_w, x = r - y * ep.in_w;
+    const int pd = ep.pad, ld = ep.lead < 0 ? ep.pad : ep.lead;
+    valid = valid && y >= ld && y < ep.in_h - pd && x >= ld && x < ep.in_w - pd;
+    if (ep.row_map == ROW_PAD2TOK) {
+      const int ho = (ep.in_h - pd - ld + ep.sub - 1) / ep.sub, wo = (ep.in_w - pd - ld + ep.sub - 1) / ep.sub;
+      valid = valid && ((y - ld) % ep.sub == 0) && ((x - ld) % ep.sub == 0);
+      drow = img * (ep.out_img_rows > 0 ? ep.out_img_rows : ho * wo) + ((y - ld) / ep.sub) * wo + (x - ld) / ep.sub;
+    } else if (ep.sub > 1 || ep.out_wp > 0) {
+      // destination geometry differs from the source one (stride-2 sub-sampling and / or another border width)
+      valid = valid && ((y - ld) % ep.sub == 0) && ((x - ld) % ep.sub == 0);
+      drow = img * ep.out_img_rows + ((y - ld) / ep.sub + out_ld) * ep.out_wp + (x - ld) / ep.sub + out_ld;
+    }
+  } else if (ep.row_map == ROW_TOKSKIP) {
+    drow = m + m / ep.in_w + 1;
+  } else if (ep.row_map == ROW_TOK2PAD || ep.row_map == ROW_SHUFFLE) {
+    const int per = ep.in_w * ep.in_h;
+    const int img = m / per, r = m - img * per;
+    ty = r / ep.in_w; tx = r - ty * ep.in_w;
+    img_base = img * ep.out_img_rows;
+    drow = img_base + (ty + out_ld) * ep.out_wp + tx + out_ld;
+  }
+  s.m = m;
+  s.valid = valid;
+  s.okrows = 0;
+#pragma unroll
+  for (int rr = 0; rr < 8; ++rr) {
+    const int row = rr * 4 + rsub;
+    s.okrows |= (__shfl_sync(0xffffffffu, valid, row) ? 1u : 0u) << rr;
+    s.dr8[rr] = __shfl_sync(0xffffffffu, drow, row);
+    if (ep.row_map == ROW_SHUFFLE) {
+      s.ty8[rr] = __shfl_sync(0xffffffffu, ty, row);
+      s.tx8[rr] = __shfl_sync(0xffffffffu, tx, row);
+      s.ib8[rr] = __shfl_sync(0xffffffffu, img_base, row);
+    }
+  }
+}
+
+// The register epilogue of one 32-row x 32-column chunk (columns nc .. nc + 31 of the output, first row m_slab) whose raw fp32
+// accumulators are in the swizzled box at shared address `box`.  `release` (may be null): an mbarrier this warp arrives on
+// once after its last shared-memory read of the chunk, before its global loads and stores.
+template <bool GRU>
+__device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& ep, int N, const SlabRows& s, uint32_t box, int nc, int m_slab,
+                                               int lane, uint64_t* release) {
+  if (ep.head_w != nullptr) {
+    // fused DPT output head (N == 32): the lane's own row, all 32 columns
+    float4 q[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) q[j] = lds128(box + lane * 128 + ((j ^ (lane & 7)) << 4));
+    if (release != nullptr) { __syncwarp(); if (lane == 0) mbar_arrive(release); }
+    if (s.valid) {
+      float acc_h = ep.head_b;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float r4[4] = {q[j].x, q[j].y, q[j].z, q[j].w};
+#pragma unroll
+        for (int t = 0; t < 4; ++t) acc_h = fmaf(fmaxf(r4[t] + __ldg(ep.bias + 4 * j + t), 0.f), __ldg(ep.head_w + 4 * j + t), acc_h);
+      }
+      int img = 0, rpix = s.m;
+      if (ep.img_rows > 0) { img = s.m / ep.img_rows; rpix = s.m - img * ep.img_rows; }
+      const int y = rpix / ep.in_w, x = rpix - y * ep.in_w, pd = ep.pad;
+      const size_t pix = ((size_t)img * (ep.in_h - 2 * pd) + (y - pd)) * (ep.in_w - 2 * pd) + (x - pd);
+      ep.head_out[pix] = fmaxf(acc_h, 0.f);
+      if (ep.out_f16) {  // also keep the 32 ReLU'd activations (the out_conv hook of the metric head), dense rows
+        uint4* dst = reinterpret_cast<uint4*>(ep.out_f16 + pix * ep.out_f16_ld);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float4 a = q[2 * j], b = q[2 * j + 1];
+          const float* bs = ep.bias + 8 * j;
+          dst[j] = make_uint4(pack_half2(fmaxf(a.x + __ldg(bs), 0.f), fmaxf(a.y + __ldg(bs + 1), 0.f)),
+                              pack_half2(fmaxf(a.z + __ldg(bs + 2), 0.f), fmaxf(a.w + __ldg(bs + 3), 0.f)),
+                              pack_half2(fmaxf(b.x + __ldg(bs + 4), 0.f), fmaxf(b.y + __ldg(bs + 5), 0.f)),
+                              pack_half2(fmaxf(b.z + __ldg(bs + 6), 0.f), fmaxf(b.w + __ldg(bs + 7), 0.f)));
+        }
+      }
+    }
+    return;
+  }
+  // ---- coalesced phase: 8 lanes x 4 columns cover one row's 32 columns; 4 rows per step
+  const int cg = lane & 7;     // which 4-column group of the 32-column chunk
+  const int rsub = lane >> 3;  // row offset inside a 4-row step
+  const int n = nc + cg * 4;
+  const bool ncol_ok = n < N;
+  float4 v[8];
+#pragma unroll
+  for (int rr = 0; rr < 8; ++rr) {
+    const int row = rr * 4 + rsub;
+    v[rr] = lds128(box + row * 128 + ((cg ^ (row & 7)) << 4));
+  }
+  if (release != nullptr) { __syncwarp(); if (lane == 0) mbar_arrive(release); }
+  float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f), gamma4 = make_float4(1.f, 1.f, 1.f, 1.f);
+  if (ncol_ok && ep.bias) bias4 = *reinterpret_cast<const float4*>(ep.bias + n);
+  if (ncol_ok && ep.gamma) gamma4 = *reinterpret_cast<const float4*>(ep.gamma + n);
+  int col = n;
+  if (ep.row_map == ROW_SHUFFLE) {
+    const int out_ld = ep.out_lead < 0 ? ep.out_pad : ep.out_lead;
+    const int q = n / ep.shuf_cout;
+    col = n - q * ep.shuf_cout;
+    const int sdy = q / ep.shuf_s, sdx = q - sdy * ep.shuf_s;
+    int drs[8];
+#pragma unroll
+    for (int rr = 0; rr < 8; ++rr)
+      drs[rr] = s.ib8[rr] + (s.ty8[rr] * ep.shuf_s + sdy + out_ld) * ep.out_wp + s.tx8[rr] * ep.shuf_s + sdx + out_ld;
+    epilogue_rows8<GRU>(ep, v, drs, ncol_ok ? s.okrows : 0u, bias4, gamma4, col);
+  } else {
+    epilogue_rows8<GRU>(ep, v, s.dr8, ncol_ok ? s.okrows : 0u, bias4, gamma4, col);
+  }
+  if (ep.stat_part != nullptr) {
+    float4 sm = make_float4(0.f, 0.f, 0.f, 0.f), sq = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int rr = 0; rr < 8; ++rr)
+      if ((s.okrows >> rr) & 1) {
+        sm.x += v[rr].x; sm.y += v[rr].y; sm.z += v[rr].z; sm.w += v[rr].w;
+        sq.x = fmaf(v[rr].x, v[rr].x, sq.x); sq.y = fmaf(v[rr].y, v[rr].y, sq.y);
+        sq.z = fmaf(v[rr].z, v[rr].z, sq.z); sq.w = fmaf(v[rr].w, v[rr].w, sq.w);
+      }
+#pragma unroll
+    for (int o = 8; o <= 16; o <<= 1) {  // the 4 lanes that hold the same 4 columns (rows rsub, rsub + 4, ...)
+      sm.x += __shfl_xor_sync(0xffffffffu, sm.x, o); sm.y += __shfl_xor_sync(0xffffffffu, sm.y, o);
+      sm.z += __shfl_xor_sync(0xffffffffu, sm.z, o); sm.w += __shfl_xor_sync(0xffffffffu, sm.w, o);
+      sq.x += __shfl_xor_sync(0xffffffffu, sq.x, o); sq.y += __shfl_xor_sync(0xffffffffu, sq.y, o);
+      sq.z += __shfl_xor_sync(0xffffffffu, sq.z, o); sq.w += __shfl_xor_sync(0xffffffffu, sq.w, o);
+    }
+    if (rsub == 0 && ncol_ok) {
+      const size_t sl = (size_t)m_slab >> 5;
+      *reinterpret_cast<float4*>(ep.stat_part + (sl * 2) * N + n) = sm;
+      *reinterpret_cast<float4*>(ep.stat_part + (sl * 2 + 1) * N + n) = sq;
+    }
+  }
+}
+
 template <int BN, bool TMAST, bool TF32>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(GemmCfg<BN, TMAST, TF32>::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmD, const __grid_constant__ GemmArgs args) {
-  using Cfg = GemmCfg<BN, TMAST>;
+  using Cfg = GemmCfg<BN, TMAST, TF32>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int BKE = TF32 ? 32 : 64;  // elements per 128-byte K block (fp32 containers for tf32, fp16 otherwise)
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -346,6 +520,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::STG_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
+  uint64_t* hfull = bars + 2 * STAGES;   // EPI_WG: the hand-off buffer holds accumulators (one arrival per consumer warp)
+  uint64_t* hempty = hfull + 1;          // EPI_WG: the hand-off buffer has been read (one arrival per epilogue warp)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -355,6 +531,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }  // empty: one arrival per consumer warpgroup
+    if (Cfg::EPI_WG) { mbar_init(hfull, 8); mbar_init(hempty, 4); }
     fence_mbar_init();
   }
   __syncthreads();
@@ -372,7 +549,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   if (wg == 2) {
     // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<Cfg::REGS_PRODUCER>();
     if (threadIdx.x == 256) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -390,18 +567,38 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
+  } else if (wg == 3) {
+    // ------------------------------------------------------------------ epilogue warpgroup (EPI_WG): warp w stores slab w
+    if constexpr (Cfg::EPI_WG) {
+      setmaxnreg_inc<Cfg::REGS_EPILOGUE>();
+      const int slab = warp & 3;
+      const uint32_t hbuf = smem_u32(stg_all) + slab * (BN / 32) * 4096;
+      uint32_t hcnt = 0;  // tiles received so far (barrier parity)
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++hcnt) {
+        int tm, tn;
+        tile_mn(tile, &tm, &tn);
+        const int m_slab = tm * GEMM_BM + slab * 32, n0 = tn * BN;
+        SlabRows rows;
+        map_slab_rows(args.ep, args.M, m_slab, lane, rows);
+        const int chunks = min(BN, args.N - n0 + 31) / 32;  // 32-column chunks holding columns < N (at least 1)
+        mbar_wait(hfull, hcnt & 1);
+#pragma unroll 1
+        for (int c = 0; c < chunks; ++c)
+          epilogue_chunk<true>(args.ep, args.N, rows, hbuf + c * 4096, n0 + c * 32, m_slab, lane, c == chunks - 1 ? hempty : nullptr);
+      }
+    }
   } else {
-    // ------------------------------------------------------------------ consumers: MMA + epilogue of 64 rows each
-    setmaxnreg_inc<232>();
+    // ------------------------------------------------------------------ consumers: MMA (+ the epilogue of 64 rows each)
+    setmaxnreg_inc<Cfg::REGS_CONSUMER>();
     const int slab = warp >> 1;    // 32-row slab of the tile this warp pair stores (0..3)
     const int half = warp & 1;     // which 32-column chunk of a 64-column block this warp stores
     const int pair_bar = 1 + slab;
     const GemmEpilogue& ep = args.ep;
     const uint32_t stg = smem_u32(stg_all) + warp * Cfg::STG_WARP;
     const uint32_t stg_pair = smem_u32(stg_all) + (warp & ~1) * Cfg::STG_WARP;
+    const uint32_t hbuf = smem_u32(stg_all) + slab * (BN / 32) * 4096;  // EPI_WG: this slab's boxes of the hand-off buffer
     uint32_t st_cnt = 0;  // TMAST: boxes stored so far by this warp (staging buffer parity)
-    const int cg = lane & 7;     // coalesced phase: which 4-column group of the 32-column chunk
-    const int rsub = lane >> 3;  // coalesced phase: row offset inside a 4-row step
+    uint32_t hcnt = 0;    // EPI_WG: tiles handed off so far (barrier parity)
     float acc[BN / 2];
     float run[TF32 ? BN / 2 : 1];
     int stage = 0; uint32_t phase = 0;
@@ -494,53 +691,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         continue;
       }
 
-      // ---- row mapping of the 32 output rows of this warp pair's slab (lane == row inside the slab)
-      int m = 0, valid = 0, drow = 0;
-      int ty = 0, tx = 0, img_base = 0;  // token coordinates / image base row for ROW_SHUFFLE
-      const int out_ld = ep.out_lead < 0 ? ep.out_pad : ep.out_lead;  // leading border of the destination map
-      int dr8[8], ty8[8], tx8[8], ib8[8];
-      uint32_t okrows = 0;
-      {
-        m = m0 + slab * 32 + lane;
-        valid = m < args.M;
-        drow = m;
-        if (ep.row_map == ROW_PADDED || ep.row_map == ROW_PAD2TOK) {
-          int img = 0, r = m;
-          if (ep.img_rows > 0) { img = m / ep.img_rows; r = m - img * ep.img_rows; }
-          const int y = r / ep.in_w, x = r - y * ep.in_w;
-          const int pd = ep.pad, ld = ep.lead < 0 ? ep.pad : ep.lead;
-          valid = valid && y >= ld && y < ep.in_h - pd && x >= ld && x < ep.in_w - pd;
-          if (ep.row_map == ROW_PAD2TOK) {
-            const int ho = (ep.in_h - pd - ld + ep.sub - 1) / ep.sub, wo = (ep.in_w - pd - ld + ep.sub - 1) / ep.sub;
-            valid = valid && ((y - ld) % ep.sub == 0) && ((x - ld) % ep.sub == 0);
-            drow = img * (ep.out_img_rows > 0 ? ep.out_img_rows : ho * wo) + ((y - ld) / ep.sub) * wo + (x - ld) / ep.sub;
-          } else if (ep.sub > 1 || ep.out_wp > 0) {
-            // destination geometry differs from the source one (stride-2 sub-sampling and / or another border width)
-            valid = valid && ((y - ld) % ep.sub == 0) && ((x - ld) % ep.sub == 0);
-            drow = img * ep.out_img_rows + ((y - ld) / ep.sub + out_ld) * ep.out_wp + (x - ld) / ep.sub + out_ld;
-          }
-        } else if (ep.row_map == ROW_TOKSKIP) {
-          drow = m + m / ep.in_w + 1;
-        } else if (ep.row_map == ROW_TOK2PAD || ep.row_map == ROW_SHUFFLE) {
-          const int per = ep.in_w * ep.in_h;
-          const int img = m / per, r = m - img * per;
-          ty = r / ep.in_w; tx = r - ty * ep.in_w;
-          img_base = img * ep.out_img_rows;
-          drow = img_base + (ty + out_ld) * ep.out_wp + tx + out_ld;
-        }
-        // row mapping of the 8 rows this lane stores in the coalesced phase
+      if constexpr (Cfg::EPI_WG) {
+        // ---- hand the raw accumulators to the epilogue warpgroup and go on to the next tile
+        mbar_wait(hempty, (hcnt & 1) ^ 1);  // the epilogue warps have read the previous tile
 #pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          const int row = rr * 4 + rsub;
-          okrows |= (__shfl_sync(0xffffffffu, valid, row) ? 1u : 0u) << rr;
-          dr8[rr] = __shfl_sync(0xffffffffu, drow, row);
-          if (ep.row_map == ROW_SHUFFLE) {
-            ty8[rr] = __shfl_sync(0xffffffffu, ty, row);
-            tx8[rr] = __shfl_sync(0xffffffffu, tx, row);
-            ib8[rr] = __shfl_sync(0xffffffffu, img_base, row);
-          }
-        }
+        for (int cb = 0; cb < BN; cb += 64) stage_fragment<BN, 0>(acc, cb, hbuf + cb / 32 * 4096, 4096, ep, n0, args.N, warp, lane);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(hfull);
+        ++hcnt;
+        continue;
       }
+
+      // ---- consumer-run register epilogue (3xTF32, 256-wide fp16 tiles): the warp pair exchanges fragments so that each warp owns 32 columns
+      SlabRows rows;
+      map_slab_rows(ep, args.M, m0 + slab * 32, lane, rows);
 #pragma unroll 1
       for (int cb = 0; cb < BN && n0 + cb < args.N; cb += 64) {
         named_bar_sync(pair_bar, 64);  // the partner has finished reading its buffer
@@ -548,85 +712,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         named_bar_sync(pair_bar, 64);
         const int c0 = cb + half * 32;
         if (c0 >= BN || n0 + c0 >= args.N) continue;  // warp-uniform
-        if (ep.head_w != nullptr) {
-          // fused DPT output head (N == 32): the lane's own row, all 32 columns
-          if (valid) {
-            float acc_h = ep.head_b;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 q = lds128(stg + lane * 128 + ((j ^ (lane & 7)) << 4));
-              const float r4[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-              for (int t = 0; t < 4; ++t) acc_h = fmaf(fmaxf(r4[t] + __ldg(ep.bias + 4 * j + t), 0.f), __ldg(ep.head_w + 4 * j + t), acc_h);
-            }
-            int img = 0, rpix = m;
-            if (ep.img_rows > 0) { img = m / ep.img_rows; rpix = m - img * ep.img_rows; }
-            const int y = rpix / ep.in_w, x = rpix - y * ep.in_w, pd = ep.pad;
-            const size_t pix = ((size_t)img * (ep.in_h - 2 * pd) + (y - pd)) * (ep.in_w - 2 * pd) + (x - pd);
-            ep.head_out[pix] = fmaxf(acc_h, 0.f);
-            if (ep.out_f16) {  // also keep the 32 ReLU'd activations (the out_conv hook of the metric head), dense rows
-              uint4* dst = reinterpret_cast<uint4*>(ep.out_f16 + pix * ep.out_f16_ld);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float4 a = lds128(stg + lane * 128 + (((2 * j) ^ (lane & 7)) << 4));
-                const float4 b = lds128(stg + lane * 128 + (((2 * j + 1) ^ (lane & 7)) << 4));
-                const float* bs = ep.bias + 8 * j;
-                dst[j] = make_uint4(pack_half2(fmaxf(a.x + __ldg(bs), 0.f), fmaxf(a.y + __ldg(bs + 1), 0.f)),
-                                    pack_half2(fmaxf(a.z + __ldg(bs + 2), 0.f), fmaxf(a.w + __ldg(bs + 3), 0.f)),
-                                    pack_half2(fmaxf(b.x + __ldg(bs + 4), 0.f), fmaxf(b.y + __ldg(bs + 5), 0.f)),
-                                    pack_half2(fmaxf(b.z + __ldg(bs + 6), 0.f), fmaxf(b.w + __ldg(bs + 7), 0.f)));
-              }
-            }
-          }
-          continue;
-        }
-        // ---- coalesced phase: 8 lanes x 4 columns cover one row's 32 columns; 4 rows per step
-        const int n = n0 + c0 + cg * 4;
-        const bool ncol_ok = n < args.N;
-        float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f), gamma4 = make_float4(1.f, 1.f, 1.f, 1.f);
-        if (ncol_ok && ep.bias) bias4 = *reinterpret_cast<const float4*>(ep.bias + n);
-        if (ncol_ok && ep.gamma) gamma4 = *reinterpret_cast<const float4*>(ep.gamma + n);
-        float4 v[8];
-#pragma unroll
-        for (int rr = 0; rr < 8; ++rr) {
-          const int row = rr * 4 + rsub;
-          v[rr] = lds128(stg + row * 128 + ((cg ^ (row & 7)) << 4));
-        }
-        int col = n;
-        if (ep.row_map == ROW_SHUFFLE) {
-          const int q = n / ep.shuf_cout;
-          col = n - q * ep.shuf_cout;
-          const int sdy = q / ep.shuf_s, sdx = q - sdy * ep.shuf_s;
-          int drs[8];
-#pragma unroll
-          for (int rr = 0; rr < 8; ++rr)
-            drs[rr] = ib8[rr] + (ty8[rr] * ep.shuf_s + sdy + out_ld) * ep.out_wp + tx8[rr] * ep.shuf_s + sdx + out_ld;
-          epilogue_rows8<!TF32>(ep, v, drs, ncol_ok ? okrows : 0u, bias4, gamma4, col);
-        } else {
-          epilogue_rows8<!TF32>(ep, v, dr8, ncol_ok ? okrows : 0u, bias4, gamma4, col);
-        }
-        if (ep.stat_part != nullptr) {
-          float4 sm = make_float4(0.f, 0.f, 0.f, 0.f), sq = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int rr = 0; rr < 8; ++rr)
-            if ((okrows >> rr) & 1) {
-              sm.x += v[rr].x; sm.y += v[rr].y; sm.z += v[rr].z; sm.w += v[rr].w;
-              sq.x = fmaf(v[rr].x, v[rr].x, sq.x); sq.y = fmaf(v[rr].y, v[rr].y, sq.y);
-              sq.z = fmaf(v[rr].z, v[rr].z, sq.z); sq.w = fmaf(v[rr].w, v[rr].w, sq.w);
-            }
-#pragma unroll
-          for (int o = 8; o <= 16; o <<= 1) {  // the 4 lanes that hold the same 4 columns (rows rsub, rsub + 4, ...)
-            sm.x += __shfl_xor_sync(0xffffffffu, sm.x, o); sm.y += __shfl_xor_sync(0xffffffffu, sm.y, o);
-            sm.z += __shfl_xor_sync(0xffffffffu, sm.z, o); sm.w += __shfl_xor_sync(0xffffffffu, sm.w, o);
-            sq.x += __shfl_xor_sync(0xffffffffu, sq.x, o); sq.y += __shfl_xor_sync(0xffffffffu, sq.y, o);
-            sq.z += __shfl_xor_sync(0xffffffffu, sq.z, o); sq.w += __shfl_xor_sync(0xffffffffu, sq.w, o);
-          }
-          if (rsub == 0 && ncol_ok) {
-            const size_t sl = (size_t)(m0 + slab * 32) >> 5;
-            *reinterpret_cast<float4*>(ep.stat_part + (sl * 2) * args.N + n) = sm;
-            *reinterpret_cast<float4*>(ep.stat_part + (sl * 2 + 1) * args.N + n) = sq;
-          }
-        }
+        epilogue_chunk<!TF32>(ep, args.N, rows, stg, n0 + c0, m0 + slab * 32, lane, nullptr);
       }
     }
     if (TMAST && lane == 0) tma_store_wait_all();  // shared memory must outlive the last bulk stores
@@ -658,6 +744,6 @@ int gemm_prepare(GemmLaunch* out, const __half* A, long long a_rows, int a_cols,
 int gemm_prepare_tf32x3(GemmLaunch* out, const float* A_split, long long a_rows, int C, int C_half, const float* W3, int w_rows,
                         int M, int N, int taps, const int* tap_off, const GemmEpilogue& ep, int num_sms, int force_bn = 0);
 int gemm_run(const GemmLaunch& g, cudaStream_t stream);
-int gemm_pick_bn(int M, int N, int num_sms);
+int gemm_pick_bn(int M, int N, int num_sms, bool epi_overlap = false);  // epi_overlap: fp16 register epilogue
 
 }  // namespace prisma
