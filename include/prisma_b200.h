@@ -205,7 +205,11 @@ int prisma_mask_work(prisma_engine* e, int h, int w, double* out8);
  * mask_mmdet (mmcv.imrescale (1333, 800)).  Pure host arithmetic, usable without a GPU.                              */
 int prisma_net_size(const char* band, int w, int h, int* wn, int* hn);
 
-/* ---- kernel-level entry points (parity tests and micro-benchmarks call the kernels through the C ABI) ---- */
+/* ---- kernel-level entry points (parity tests and micro-benchmarks call the kernels through the C ABI) ----
+ * The ViT-encoder and DPT-resampler entries (attention[_batch], layernorm[_skip], pos_embed, patchify, readout_concat, upsample_ac,
+ * upsample_bicubic; tests/test_vit_kernels_gpu.py) take host arrays only: they check every argument before touching the
+ * device (a bad one returns < 0 and prisma_last_error() names it), allocate all device buffers from the dimensions, fill
+ * the destination with all-ones bytes (NaN in fp16 and fp32) before the launch and return all of it, borders included. */
 /* D = A[M,K] * W[N,K]^T (+bias) with fp16 operands / fp32 accumulate on the wgmma core; A, W, D host fp32.
  * act: 0 none, 1 gelu, 2 relu (register epilogue, fp32 out); TMA-store epilogues: -4 fp32 out, no bias, accumulator scaled
  * by 1/16 (the RAFT correlation path); -5 the same with an fp16 destination; -6 / -7 fp16 out with bias + GELU / ReLU (the
@@ -266,9 +270,29 @@ int prisma_debug_gemm_tf32x3(int device, const float* A, const float* W, const f
 /* 3x3 (kh x kw) stride-1 'same' convolution, NHWC fp32 host in/out, through the shifted-row GEMM.           */
 int prisma_debug_conv(int device, const float* x_nhwc, const float* w_oihw, const float* bias, float* y_nhwc, int H,
                       int W, int Cin, int Cout, int kh, int kw, int relu, float* ms_out);
-/* softmax(q k^T) v per head (head_dim 64); qkv host fp32 [T][3*D] (q NOT pre-scaled; scaled inside), out [T][D] */
+/* softmax(q k^T) v per image and head (head_dim 64, D = 64 * heads); qkv host fp32 [batch*T][3*D] (q NOT pre-scaled; scaled
+ * inside), out [batch*T][D].  prisma_debug_attention is the same with batch = 1.                                        */
+int prisma_debug_attention_batch(int device, const float* qkv, float* out, int batch, int T, int heads, int iters,
+                                 float* ms_out);
 int prisma_debug_attention(int device, const float* qkv, float* out, int T, int heads, int iters, float* ms_out);
+/* LayerNorm (eps 1e-6) fp32 -> fp16, D in {384, 768, 1024}: y [rows][D]; skip_per > 0 reads x [rows/skip_per*(skip_per+1)][D]
+ * and drops the first row of every group of skip_per + 1 (the cls token; the engine's ln_out).  prisma_debug_layernorm is
+ * the same with skip_per = 0.                                                                                             */
+int prisma_debug_layernorm_skip(int device, const float* x, const float* g, const float* b, float* y, int rows, int D,
+                                int skip_per);
 int prisma_debug_layernorm(int device, const float* x, const float* g, const float* b, float* y, int rows, int D);
+/* da_pos_embed: pos [1+S*S][D], cls [D] -> out [1+ph*pw][D] = (pos[0] + cls, the S x S grid resampled to ph x pw)     */
+int prisma_debug_pos_embed(int device, const float* pos, const float* cls, int S, int D, int ph, int pw, float* out);
+/* da_patchify: x [B][3][h][w] -> out [B*P][kpad] (fp16 values as fp32), P = (h/patch)*(w/patch), kpad = round_up(3*patch^2, 64) */
+int prisma_debug_patchify(int device, const float* x, int B, int h, int w, int patch, float* out);
+/* readout_concat_f16: x [B*T][D] -> out [B*(T-1)][2D] = [token | cls of its image] (fp16 values as fp32)                 */
+int prisma_debug_readout_concat(int device, const float* x, int B, int T, int D, float* out);
+/* upsample_ac_f16 (bilinear, align_corners=True): in [B][ih][iw][C] -> out, out_relu [B][oh+2][ow+2][C] zero-bordered maps
+ * (fp16 values as fp32); out_relu = max(out, 0) when relu_copy != 0, else left as filled                                */
+int prisma_debug_upsample_ac(int device, const float* in, int B, int ih, int iw, int C, int oh, int ow, int relu_copy,
+                             float* out, float* out_relu);
+/* upsample_bicubic_ac_f32 (bicubic, align_corners=True): in [ih][iw] -> out [oh][ow], fp32                              */
+int prisma_debug_upsample_bicubic(int device, const float* in, int ih, int iw, float* out, int oh, int ow);
 /* OpenCV-exact cubic resize + normalise (K1): rgb u8 h*w*3 -> f32 [3][hn][wn]                                */
 int prisma_debug_da_preprocess(int device, const uint8_t* rgb, int h, int w, float* out, int hn, int wn);
 

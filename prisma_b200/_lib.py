@@ -105,7 +105,15 @@ SIGNATURES = {
     "prisma_debug_conv": (C.c_int, [C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
     "prisma_debug_attention": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_attention_batch": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
     "prisma_debug_layernorm": (C.c_int, [C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int]),
+    "prisma_debug_layernorm_skip": (C.c_int, [C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int]),
+    "prisma_debug_pos_embed": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_patchify": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_readout_concat": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_upsample_ac": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                           c_float_p, c_float_p]),
+    "prisma_debug_upsample_bicubic": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, c_float_p, C.c_int, C.c_int]),
     "prisma_debug_da_preprocess": (C.c_int, [C.c_int, c_u8_p, C.c_int, C.c_int, c_float_p, C.c_int, C.c_int]),
 }
 

@@ -452,47 +452,223 @@ int prisma_debug_conv(int device, const float* x, const float* w_oihw, const flo
   API_GUARD_END
 }
 
-int prisma_debug_attention(int device, const float* qkv, float* out, int T, int heads, int iters, float* ms_out) {
+// Kernel-level entries of the ViT encoder and the DPT resamplers.  Each one checks its arguments before it touches the device
+// (so a refusal needs no GPU), allocates every device buffer from the dimensions, fills the destination with all-ones bytes
+// (NaN in fp16 and fp32) before the launch, and returns the whole destination, borders and padding included, so a caller
+// can tell which cells the kernel wrote.
+#define DEBUG_ARG(cond, fn, arg, what) PRISMA_CHECK(cond, fn ": bad argument `" arg "`: " what)
+
+int prisma_debug_attention_batch(int device, const float* qkv, float* out, int batch, int T, int heads, int iters,
+                                 float* ms_out) {
   API_GUARD_BEGIN
+  DEBUG_ARG(qkv != nullptr, "prisma_debug_attention_batch", "qkv", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_attention_batch", "out", "NULL");
+  DEBUG_ARG(batch >= 1, "prisma_debug_attention_batch", "batch", "must be >= 1");
+  DEBUG_ARG(T >= 1, "prisma_debug_attention_batch", "T", "must be >= 1");
+  DEBUG_ARG(heads >= 1 && heads <= 64, "prisma_debug_attention_batch", "heads", "must be in [1, 64]");
+  DEBUG_ARG((long long)batch * T <= (1 << 24), "prisma_debug_attention_batch", "T", "batch * T must be at most 2^24 rows");
   int sms = 0;
   PRISMA_TRY(device_sms(device, &sms));
   const int D = heads * 64;
+  const size_t rows = (size_t)batch * T;
   Scratch sc;
-  std::vector<__half> h((size_t)T * 3 * D);
-  for (int t = 0; t < T; ++t)
+  std::vector<__half> h(rows * 3 * D);
+  for (size_t t = 0; t < rows; ++t)
     for (int c = 0; c < 3 * D; ++c)
-      h[(size_t)t * 3 * D + c] = __float2half_rn(qkv[(size_t)t * 3 * D + c] * (c < D ? 0.125f : 1.f));
+      h[t * 3 * D + c] = __float2half_rn(qkv[t * 3 * D + c] * (c < D ? 0.125f : 1.f));
   __half* dq = sc.alloc<__half>(h.size());
-  __half* dO = sc.alloc<__half>((size_t)T * D);
+  __half* dO = sc.alloc<__half>(rows * D);
   PRISMA_CHECK(dq && dO, "cudaMalloc failed");
   PRISMA_CUDA_OK(cudaMemcpy(dq, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dO, 0xFF, rows * D * 2));
   AttnLaunch a;
-  PRISMA_TRY(attention_prepare(&a, dq, dO, 1, T, heads, D));
+  PRISMA_TRY(attention_prepare(&a, dq, dO, batch, T, heads, D));
   PRISMA_TRY(timed(0, iters > 0 ? iters : 1, ms_out, [&]() { return attention_run(a, 0); }));
-  std::vector<__half> ho((size_t)T * D);
+  std::vector<__half> ho(rows * D);
   PRISMA_CUDA_OK(cudaMemcpy(ho.data(), dO, ho.size() * 2, cudaMemcpyDeviceToHost));
   for (size_t i = 0; i < ho.size(); ++i) out[i] = __half2float(ho[i]);
   return 0;
   API_GUARD_END
 }
 
-int prisma_debug_layernorm(int device, const float* x, const float* g, const float* b, float* y, int rows, int D) {
+int prisma_debug_layernorm_skip(int device, const float* x, const float* g, const float* b, float* y, int rows, int D,
+                                int skip_per) {
   API_GUARD_BEGIN
+  DEBUG_ARG(x != nullptr, "prisma_debug_layernorm_skip", "x", "NULL");
+  DEBUG_ARG(g != nullptr, "prisma_debug_layernorm_skip", "g", "NULL");
+  DEBUG_ARG(b != nullptr, "prisma_debug_layernorm_skip", "b", "NULL");
+  DEBUG_ARG(y != nullptr, "prisma_debug_layernorm_skip", "y", "NULL");
+  DEBUG_ARG(rows >= 1, "prisma_debug_layernorm_skip", "rows", "must be >= 1");
+  DEBUG_ARG(D == 384 || D == 768 || D == 1024, "prisma_debug_layernorm_skip", "D", "must be 384, 768 or 1024");
+  DEBUG_ARG(skip_per >= 0, "prisma_debug_layernorm_skip", "skip_per", "must be >= 0");
+  DEBUG_ARG(skip_per == 0 || rows % skip_per == 0, "prisma_debug_layernorm_skip", "skip_per", "rows must be a multiple of it");
   int sms = 0;
   PRISMA_TRY(device_sms(device, &sms));
+  // skip_per > 0: every group of skip_per output rows reads skip_per + 1 input rows and drops the first (the cls token)
+  const size_t in_rows = skip_per > 0 ? (size_t)(rows / skip_per) * (skip_per + 1) : (size_t)rows;
   Scratch sc;
-  float* dx = sc.alloc<float>((size_t)rows * D);
+  float* dx = sc.alloc<float>(in_rows * D);
   float* dg = sc.alloc<float>(D);
   float* db = sc.alloc<float>(D);
   __half* dy = sc.alloc<__half>((size_t)rows * D);
   PRISMA_CHECK(dx && dg && db && dy, "cudaMalloc failed");
-  PRISMA_CUDA_OK(cudaMemcpy(dx, x, (size_t)rows * D * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dx, x, in_rows * D * 4, cudaMemcpyHostToDevice));
   PRISMA_CUDA_OK(cudaMemcpy(dg, g, D * 4, cudaMemcpyHostToDevice));
   PRISMA_CUDA_OK(cudaMemcpy(db, b, D * 4, cudaMemcpyHostToDevice));
-  PRISMA_TRY(layernorm_f16(dx, dg, db, dy, rows, D, 1e-6f, 0));
+  PRISMA_CUDA_OK(cudaMemset(dy, 0xFF, (size_t)rows * D * 2));
+  PRISMA_TRY(layernorm_f16(dx, dg, db, dy, rows, D, 1e-6f, 0, skip_per));
   std::vector<__half> hy((size_t)rows * D);
   PRISMA_CUDA_OK(cudaMemcpy(hy.data(), dy, hy.size() * 2, cudaMemcpyDeviceToHost));
   for (size_t i = 0; i < hy.size(); ++i) y[i] = __half2float(hy[i]);
+  return 0;
+  API_GUARD_END
+}
+
+// The single-image / dense-row forms keep their original signatures for existing callers.
+int prisma_debug_attention(int device, const float* qkv, float* out, int T, int heads, int iters, float* ms_out) {
+  return prisma_debug_attention_batch(device, qkv, out, 1, T, heads, iters, ms_out);
+}
+int prisma_debug_layernorm(int device, const float* x, const float* g, const float* b, float* y, int rows, int D) {
+  return prisma_debug_layernorm_skip(device, x, g, b, y, rows, D, 0);
+}
+
+int prisma_debug_pos_embed(int device, const float* pos, const float* cls, int S, int D, int ph, int pw, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(pos != nullptr, "prisma_debug_pos_embed", "pos", "NULL");
+  DEBUG_ARG(cls != nullptr, "prisma_debug_pos_embed", "cls", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_pos_embed", "out", "NULL");
+  DEBUG_ARG(S >= 1 && S <= 1024, "prisma_debug_pos_embed", "S", "must be in [1, 1024]");
+  DEBUG_ARG(D >= 4 && D % 4 == 0 && D <= 4096, "prisma_debug_pos_embed", "D", "must be a multiple of 4 in [4, 4096]");
+  DEBUG_ARG(ph >= 1 && ph <= 1024, "prisma_debug_pos_embed", "ph", "must be in [1, 1024]");
+  DEBUG_ARG(pw >= 1 && pw <= 1024, "prisma_debug_pos_embed", "pw", "must be in [1, 1024]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_in = (size_t)(1 + S * S) * D, n_out = (size_t)(1 + ph * pw) * D;
+  Scratch sc;
+  float* dpos = sc.alloc<float>(n_in);
+  float* dcls = sc.alloc<float>(D);
+  float* dout = sc.alloc<float>(n_out);
+  PRISMA_CHECK(dpos && dcls && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dpos, pos, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dcls, cls, (size_t)D * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 4));
+  PRISMA_TRY(da_pos_embed(dpos, dcls, S, D, ph, pw, dout, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(out, dout, n_out * 4, cudaMemcpyDeviceToHost));
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_patchify(int device, const float* x, int B, int h, int w, int patch, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(x != nullptr, "prisma_debug_patchify", "x", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_patchify", "out", "NULL");
+  DEBUG_ARG(B >= 1, "prisma_debug_patchify", "B", "must be >= 1");
+  DEBUG_ARG(patch >= 1 && patch <= 32, "prisma_debug_patchify", "patch", "must be in [1, 32]");
+  DEBUG_ARG(h >= patch && h <= 8192, "prisma_debug_patchify", "h", "must be in [patch, 8192]");
+  DEBUG_ARG(w >= patch && w <= 8192, "prisma_debug_patchify", "w", "must be in [patch, 8192]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const int kpad = round_up(3 * patch * patch, 64), P = (h / patch) * (w / patch);  // the engine's row pitch
+  const size_t n_in = (size_t)B * 3 * h * w, n_out = (size_t)B * P * kpad;
+  Scratch sc;
+  float* dx = sc.alloc<float>(n_in);
+  __half* dout = sc.alloc<__half>(n_out);
+  PRISMA_CHECK(dx && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dx, x, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 2));
+  PRISMA_TRY(da_patchify(dx, B, h, w, dout, kpad, 0, patch));
+  std::vector<__half> ho(n_out);
+  PRISMA_CUDA_OK(cudaMemcpy(ho.data(), dout, n_out * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n_out; ++i) out[i] = __half2float(ho[i]);
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_readout_concat(int device, const float* x, int B, int T, int D, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(x != nullptr, "prisma_debug_readout_concat", "x", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_readout_concat", "out", "NULL");
+  DEBUG_ARG(B >= 1, "prisma_debug_readout_concat", "B", "must be >= 1");
+  DEBUG_ARG(T >= 2, "prisma_debug_readout_concat", "T", "must be >= 2 (a cls token and at least one patch token)");
+  DEBUG_ARG(D >= 4 && D % 4 == 0 && D <= 4096, "prisma_debug_readout_concat", "D", "must be a multiple of 4 in [4, 4096]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_in = (size_t)B * T * D, n_out = (size_t)B * (T - 1) * 2 * D;
+  Scratch sc;
+  float* dx = sc.alloc<float>(n_in);
+  __half* dout = sc.alloc<__half>(n_out);
+  PRISMA_CHECK(dx && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dx, x, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 2));
+  PRISMA_TRY(readout_concat_f16(dx, B, T, D, dout, 0));
+  std::vector<__half> ho(n_out);
+  PRISMA_CUDA_OK(cudaMemcpy(ho.data(), dout, n_out * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n_out; ++i) out[i] = __half2float(ho[i]);
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_upsample_ac(int device, const float* in, int B, int ih, int iw, int C, int oh, int ow, int relu_copy,
+                             float* out, float* out_relu) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(in != nullptr, "prisma_debug_upsample_ac", "in", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_upsample_ac", "out", "NULL");
+  DEBUG_ARG(out_relu != nullptr, "prisma_debug_upsample_ac", "out_relu", "NULL");
+  DEBUG_ARG(B >= 1, "prisma_debug_upsample_ac", "B", "must be >= 1");
+  DEBUG_ARG(ih >= 1 && ih <= 4096, "prisma_debug_upsample_ac", "ih", "must be in [1, 4096]");
+  DEBUG_ARG(iw >= 1 && iw <= 4096, "prisma_debug_upsample_ac", "iw", "must be in [1, 4096]");
+  DEBUG_ARG(C >= 8 && C % 8 == 0 && C <= 1024, "prisma_debug_upsample_ac", "C", "must be a multiple of 8 in [8, 1024]");
+  DEBUG_ARG(oh >= 1 && oh <= 4096, "prisma_debug_upsample_ac", "oh", "must be in [1, 4096]");
+  DEBUG_ARG(ow >= 1 && ow <= 4096, "prisma_debug_upsample_ac", "ow", "must be in [1, 4096]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  // zero-bordered NHWC maps, as the engine keeps them: [B][h + 2][w + 2][C]
+  const size_t iwp = iw + 2, owp = ow + 2;
+  const size_t n_in = (size_t)B * (ih + 2) * iwp * C, n_out = (size_t)B * (oh + 2) * owp * C;
+  std::vector<__half> hi(n_in, __float2half_rn(0.f));
+  for (int bb = 0; bb < B; ++bb)
+    for (int yy = 0; yy < ih; ++yy)
+      for (int xx = 0; xx < iw; ++xx)
+        for (int c = 0; c < C; ++c)
+          hi[(((size_t)bb * (ih + 2) + yy + 1) * iwp + xx + 1) * C + c] =
+              __float2half_rn(in[(((size_t)bb * ih + yy) * iw + xx) * C + c]);
+  Scratch sc;
+  __half* di = sc.alloc<__half>(n_in);
+  __half* dout = sc.alloc<__half>(n_out);
+  __half* drelu = sc.alloc<__half>(n_out);
+  PRISMA_CHECK(di && dout && drelu, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(di, hi.data(), n_in * 2, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 2));
+  PRISMA_CUDA_OK(cudaMemset(drelu, 0xFF, n_out * 2));
+  PRISMA_TRY(upsample_ac_f16(di, B, ih, iw, C, dout, oh, ow, relu_copy ? drelu : nullptr, 0));
+  std::vector<__half> ho(n_out);
+  PRISMA_CUDA_OK(cudaMemcpy(ho.data(), dout, n_out * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n_out; ++i) out[i] = __half2float(ho[i]);
+  PRISMA_CUDA_OK(cudaMemcpy(ho.data(), drelu, n_out * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n_out; ++i) out_relu[i] = __half2float(ho[i]);
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_upsample_bicubic(int device, const float* in, int ih, int iw, float* out, int oh, int ow) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(in != nullptr, "prisma_debug_upsample_bicubic", "in", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_upsample_bicubic", "out", "NULL");
+  DEBUG_ARG(ih >= 1 && ih <= 8192, "prisma_debug_upsample_bicubic", "ih", "must be in [1, 8192]");
+  DEBUG_ARG(iw >= 1 && iw <= 8192, "prisma_debug_upsample_bicubic", "iw", "must be in [1, 8192]");
+  DEBUG_ARG(oh >= 1 && oh <= 8192, "prisma_debug_upsample_bicubic", "oh", "must be in [1, 8192]");
+  DEBUG_ARG(ow >= 1 && ow <= 8192, "prisma_debug_upsample_bicubic", "ow", "must be in [1, 8192]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_in = (size_t)ih * iw, n_out = (size_t)oh * ow;
+  Scratch sc;
+  float* di = sc.alloc<float>(n_in);
+  float* dout = sc.alloc<float>(n_out);
+  PRISMA_CHECK(di && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(di, in, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 4));
+  PRISMA_TRY(upsample_bicubic_ac_f32(di, ih, iw, dout, oh, ow, sms, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(out, dout, n_out * 4, cudaMemcpyDeviceToHost));
   return 0;
   API_GUARD_END
 }

@@ -112,6 +112,9 @@ int da_patchify(const float* x, int batch, int h, int w, __half* out, int kpad, 
 // K3: pos-embed interpolation (once per resolution): F.interpolate(bicubic, scale_factor=((ph+.1)/S,(pw+.1)/S))
 // of the SxS grid (vision_transformer.py:179-210).  torch semantics: src = (dst+0.5)*(1/scale_factor) - 0.5 in
 // float, A=-0.75, the four taps evaluated independently, clamped reads.  out[0] = pos[0] + cls.
+// Square-grid rule: when the grid is already S x S (ph == pw == S), interpolate_pos_encoding returns the table unchanged
+// (vision_transformer.py:183-184) -- a resample with scale factor (S+0.1)/S would not be the identity -- so da_pos_embed
+// copies rows 1..S*S bit for bit and launches only the block of row 0.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float cubic1(float x, float A) { return ((A + 2.f) * x - (A + 3.f)) * x * x + 1.f; }
 __device__ __forceinline__ float cubic2(float x, float A) { return ((A * x - 5.f * A) * x + 8.f * A) * x - 4.f * A; }
@@ -151,8 +154,10 @@ int da_pos_embed(const float* pos, const float* cls, int S, int D, int ph, int p
   // torch: scale = (float)(1.0 / scale_factor), scale_factor = (p + 0.1) / S computed in double
   const float rsy = (float)(1.0 / ((double)(ph + 0.1) / (double)S));
   const float rsx = (float)(1.0 / ((double)(pw + 0.1) / (double)S));
-  k_pos_embed<<<1 + ph * pw, 128, 0, s>>>(pos, cls, S, D, ph, pw, rsy, rsx, out);
+  const bool square = ph == S && pw == S;
+  k_pos_embed<<<square ? 1 : 1 + ph * pw, 128, 0, s>>>(pos, cls, S, D, ph, pw, rsy, rsx, out);
   PRISMA_CUDA_OK(cudaGetLastError());
+  if (square) PRISMA_CUDA_OK(cudaMemcpyAsync(out + D, pos + D, (size_t)S * S * D * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return 0;
 }
 

@@ -80,3 +80,57 @@ def test_bench_b200_arm_never_imports_oracle():
                 mods.extend(a.name for a in node.names)
         bad = [m for m in mods if m.split(".")[0] == "oracle"]
         assert not bad or fn.name in allowed, (fn.name, bad)
+
+
+def test_debug_entries_refuse_bad_arguments_before_the_device(built_lib):
+    """The kernel-level entries of the ViT encoder and DPT resamplers check every argument before they touch the device:
+    each bad argument returns < 0 and prisma_last_error() names it, with or without a GPU (no launch is made here)."""
+    import ctypes as C
+    from prisma_b200._lib import fptr, lib
+    l = lib()
+    a = np.zeros(64, np.float32)
+    p, null = fptr(a), None
+    ms = C.c_float()
+    cases = {
+        "prisma_debug_attention_batch": (lambda q, o, batch, T, heads: l.prisma_debug_attention_batch(0, q, o, batch, T, heads, 1, C.byref(ms)),
+                                   dict(q=p, o=p, batch=1, T=5, heads=6),
+                                   [("qkv", dict(q=null)), ("out", dict(o=null)), ("batch", dict(batch=0)), ("T", dict(T=0)),
+                                    ("heads", dict(heads=0))]),
+        "prisma_debug_layernorm_skip": (lambda x, g, b, y, rows, D, skip: l.prisma_debug_layernorm_skip(0, x, g, b, y, rows, D, skip),
+                                   dict(x=p, g=p, b=p, y=p, rows=2738, D=384, skip=1369),
+                                   [("x", dict(x=null)), ("g", dict(g=null)), ("b", dict(b=null)), ("y", dict(y=null)),
+                                    ("rows", dict(rows=0)), ("D", dict(D=512)), ("D", dict(D=383)),
+                                    ("skip_per", dict(skip=-1)), ("skip_per", dict(skip=1368))]),
+        "prisma_debug_pos_embed": (lambda pos, cls, S, D, ph, pw, out: l.prisma_debug_pos_embed(0, pos, cls, S, D, ph, pw, out),
+                                   dict(pos=p, cls=p, S=37, D=384, ph=37, pw=66, out=p),
+                                   [("pos", dict(pos=null)), ("cls", dict(cls=null)), ("out", dict(out=null)), ("S", dict(S=0)),
+                                    ("D", dict(D=386)), ("D", dict(D=0)), ("ph", dict(ph=0)), ("pw", dict(pw=0))]),
+        "prisma_debug_patchify": (lambda x, B, h, w, patch, out: l.prisma_debug_patchify(0, x, B, h, w, patch, out),
+                                  dict(x=p, B=2, h=42, w=56, patch=14, out=p),
+                                  [("x", dict(x=null)), ("out", dict(out=null)), ("B", dict(B=0)), ("patch", dict(patch=0)),
+                                   ("h", dict(h=13)), ("w", dict(w=0))]),
+        "prisma_debug_readout_concat": (lambda x, B, T, D, out: l.prisma_debug_readout_concat(0, x, B, T, D, out),
+                                        dict(x=p, B=1, T=5, D=768, out=p),
+                                        [("x", dict(x=null)), ("out", dict(out=null)), ("B", dict(B=0)), ("T", dict(T=1)),
+                                         ("D", dict(D=770)), ("D", dict(D=0))]),
+        "prisma_debug_upsample_ac": (lambda i, B, ih, iw, Cc, oh, ow, o, r: l.prisma_debug_upsample_ac(0, i, B, ih, iw, Cc, oh, ow, 1, o, r),
+                                     dict(i=p, B=2, ih=4, iw=5, Cc=64, oh=8, ow=10, o=p, r=p),
+                                     [("in", dict(i=null)), ("out", dict(o=null)), ("out_relu", dict(r=null)), ("B", dict(B=0)),
+                                      ("ih", dict(ih=0)), ("iw", dict(iw=0)), ("C", dict(Cc=60)), ("C", dict(Cc=0)),
+                                      ("oh", dict(oh=0)), ("ow", dict(ow=-3))]),
+        "prisma_debug_upsample_bicubic": (lambda i, ih, iw, o, oh, ow: l.prisma_debug_upsample_bicubic(0, i, ih, iw, o, oh, ow),
+                                          dict(i=p, ih=224, iw=384, o=p, oh=720, ow=1280),
+                                          [("in", dict(i=null)), ("out", dict(o=null)), ("ih", dict(ih=0)), ("iw", dict(iw=0)),
+                                           ("oh", dict(oh=0)), ("ow", dict(ow=0))]),
+    }
+    for fn, (call, good, bad) in cases.items():
+        for arg, change in bad:
+            rc = call(**{**good, **change})
+            msg = l.prisma_last_error().decode()
+            assert rc < 0, (fn, arg, change)
+            assert f"{fn}: bad argument `{arg}`" in msg, (fn, arg, msg)
+    # the single-image / dense-row forms go through the same checks
+    assert l.prisma_debug_attention(0, p, p, 5, 0, 1, C.byref(ms)) < 0
+    assert "bad argument `heads`" in l.prisma_last_error().decode()
+    assert l.prisma_debug_layernorm(0, p, p, p, p, 7, 500) < 0
+    assert "bad argument `D`" in l.prisma_last_error().decode()
