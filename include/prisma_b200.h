@@ -107,8 +107,15 @@ int prisma_flowcorr_build(prisma_engine* e, int iters, float* ms_out);
 int prisma_flowcorr_lookup(prisma_engine* e, const float* coords, float* out, int iters, float* ms_out);
 /* rows [row0,row0+nrows) of pyramid level `level` of image `b`: out f32 [nrows][(h8>>level)*(w8>>level)]        */
 int prisma_flowcorr_read_level(prisma_engine* e, int level, int b, int row0, int nrows, float* out);
-/* algorithmic work of one build: out[0] = FLOP, out[1] = bytes (fp32 pyramid written + fp16 features read)      */
+/* work of one build: out[0] = FLOP, out[1] = bytes (fp32 pyramid written + fp16 features read)                */
 int prisma_flowcorr_work(prisma_engine* e, double* out2);
+/* The layout of one RAFT clip pass: npairs + 1 frames, direction 2p = frame p against p + 1, 2p + 1 = frame p + 1
+ * against p (npairs 1..4, batch = 2 * npairs directions).  Level 0 of direction 2p + 1 is stored once, as the
+ * transpose of 2p's;
+ * read_level and lookup return the same values as for a separately built volume.                                */
+int prisma_flowcorr_create_pairs(int device, int npairs, int h8, int w8, prisma_engine** out);
+/* frames: host f32 [n_frames][256][h8][w8] (create_pairs: n_frames = npairs + 1; create: 2 * batch, fmap1 then fmap2) */
+int prisma_flowcorr_set_frames(prisma_engine* e, const float* frames);
 
 /* ---- RAFT band, whole model: replaces init_model (bands/flow_raft.py:38-48) + infer (:51-66) + the resize of
  *      process_video (:100-101) + process_flow (common/encode.py:113-126) for one frame pair, forward and backward   */
@@ -157,9 +164,9 @@ long long prisma_flow_read_tap(prisma_engine* e, const char* name, float* out, l
 /* out[0] = algorithmic FLOP of one pass, out[1] = kernel launches per pass, out[2] = hs, out[3] = ws               */
 int prisma_flow_work(prisma_engine* e, int h, int w, double scale, int iters, double* out4);
 /* out[0] / out[1] = algorithmic FLOP of the wgmma conv GEMMs of the full / the video pass (encoders, update block, heads;
- * without the correlation build), out[2] / out[3] = FLOP / algorithmic bytes of one correlation-pyramid build (all 2 * pairs_per_pass
- * directions of a pass; bytes = fp32 pyramid written once + fp16 features read once, raft/corr.py:13-27), out[4] / out[5] = kernel
- * steps of the full / video pass, out[6], out[7] = hs, ws                                                              */
+ * without the correlation build), out[2] / out[3] = FLOP / bytes of one correlation-pyramid build (all 2 * pairs_per_pass
+ * directions of a pass, level 0 once per pair; bytes = fp32 pyramid written once + fp16 features read once,
+ * raft/corr.py:13-27), out[4] / out[5] = kernel steps of the full / video pass, out[6], out[7] = hs, ws              */
 int prisma_flow_work_detail(prisma_engine* e, int h, int w, double scale, int iters, double* out8);
 /* CUDA-event times (ms) of one pass by kernel group, for bench.py's roofline block (video pass when the previous call left
  * its features): out[0] pre-process, [1] conv GEMMs, [2] correlation build, [3] correlation lookup, [4] InstanceNorm,

@@ -79,6 +79,8 @@ SIGNATURES = {
     "prisma_flowcorr_lookup": (C.c_int, [C.c_void_p, c_float_p, c_float_p, C.c_int, c_float_p]),
     "prisma_flowcorr_read_level": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
     "prisma_flowcorr_work": (C.c_int, [C.c_void_p, c_double_p]),
+    "prisma_flowcorr_create_pairs": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "prisma_flowcorr_set_frames": (C.c_int, [C.c_void_p, c_float_p]),
     "prisma_flow_create": (C.c_int, [C.c_int, C.POINTER(C.c_void_p)]),
     "prisma_flow_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_float_p, c_i64_p, C.c_int]),
     "prisma_flow_finalize": (C.c_int, [C.c_void_p]),

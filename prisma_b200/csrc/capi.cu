@@ -778,6 +778,23 @@ int prisma_flowcorr_create(int device, int batch, int h8, int w8, prisma_engine*
   return 0;
   API_GUARD_END
 }
+int prisma_flowcorr_create_pairs(int device, int npairs, int h8, int w8, prisma_engine** out) {
+  API_GUARD_BEGIN
+  PRISMA_CHECK(out != nullptr, "null argument");
+  FlowCorr* c = new FlowCorr();
+  int r = c->init_pairs(device, npairs, h8, w8);
+  if (r != 0) { delete c; return r; }
+  *out = new prisma_engine{2, nullptr, c};
+  return 0;
+  API_GUARD_END
+}
+int prisma_flowcorr_set_frames(prisma_engine* e, const float* frames) {
+  API_GUARD_BEGIN
+  FlowCorr* c = as_corr(e);
+  PRISMA_CHECK(frames != nullptr, "null argument");
+  return c ? c->set_frames(frames) : -1;
+  API_GUARD_END
+}
 int prisma_flowcorr_set_fmaps(prisma_engine* e, const float* fmap1, const float* fmap2) {
   API_GUARD_BEGIN
   FlowCorr* c = as_corr(e);

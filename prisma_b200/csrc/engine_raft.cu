@@ -370,11 +370,12 @@ int RaftEngine::set_pairs_per_pass(int np) {
 }
 
 // Pairs per pass the clip path uses for frames of this size: the setting, lowered until the fp32 correlation pyramids of
-// one pass (2 np directions x P^2 x 4 bytes x 4/3) fit in a third of the device memory (4K frames: one pair per pass).
+// one pass fit in a third of the device memory (4K frames: one pair per pass).  A pair holds one level 0 (P^2 x 4 bytes,
+// the backward direction reads it transposed) and levels 1..3 of both directions (2 x 1/3 of that).
 int RaftEngine::clip_pairs(int H, int W, double scale) const {
   const int hs = (int)nearbyint((double)H * scale), ws = (int)nearbyint((double)W * scale);
   const double P = (double)((hs + 7) / 8) * ((ws + 7) / 8);
-  const double per_pair = 2.0 * P * P * 4.0 * (4.0 / 3.0);
+  const double per_pair = P * P * 4.0 * (1.0 + 2.0 / 3.0);
   int np = stream_pairs;
   while (np > 1 && per_pair * np > (double)device_mem / 3.0) --np;
   return np;
@@ -411,8 +412,6 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
   // rows of every update-block launch (four waves of tiles instead of two), halving the per-pair share of each launch's
   // fixed cost (DESIGN.md section 4.1).
   const int NP = npairs, NF = NP + 1, B = 2 * NP, P = H8 * W8;
-  int fr1[8], fr2[8];
-  for (int pp = 0; pp < NP; ++pp) { fr1[2 * pp] = pp; fr2[2 * pp] = pp + 1; fr1[2 * pp + 1] = pp + 1; fr2[2 * pp + 1] = pp; }
   plan_B = B;
 
   PRISMA_TRY(r_alloc(plan_allocs, &b.img, (size_t)NF * H * W * 3));
@@ -440,7 +439,7 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
   PRISMA_TRY(r_alloc(plan_allocs, &b.maxd, 8));
 
   corr = new FlowCorr();
-  PRISMA_TRY(corr->init(device, B, H8, W8, NF, fr1, fr2));
+  PRISMA_TRY(corr->init_pairs(device, NP, H8, W8));
 
   // ---- K11 pre-process of both frames, stem im2col (shared by fnet and cnet)
   {
@@ -500,7 +499,7 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
     PRISMA_TRY(add_conv("fnet_out", f128c, 0, w.fnet.out, ep, 1)); }
   { FlowCorr* c = corr; add("corr_pool", [=](cudaStream_t s) { return c->pool_frames(1, NP, s); }); }
   cur_mask = 3;
-  {  // direction b correlates frame fr1[b] against frame fr2[b] (flow_raft.py:105-106): the GEMMs read the per-frame features
+  {  // direction b correlates frame f1[b] against frame f2[b] (flow_raft.py:105-106): the GEMMs read the per-frame features
     FlowCorr* c = corr;
     add("corr_build", [c](cudaStream_t s) { return c->build_gemms(s); });
     flops += c->flops_build;
@@ -526,7 +525,7 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
     const float* cn = b.cnet_out; float* hm = b.h_master; __half* hxp = hx.p; __half* rhp = rhx.p; const int h8 = H8, w8 = W8;
     float* c0 = b.coords0; float* c1p = b.coords1; const long long ir8 = hx.img_rows();
     DirFrames df;  // the context features of direction b are those of its image1 frame
-    for (int d = 0; d < 8; ++d) df.f[d] = d < B ? fr1[d] : 0;
+    for (int d = 0; d < 8; ++d) df.f[d] = d < B ? corr->f1[d] : 0;
     add("cnet_split", [=](cudaStream_t s) { return raft_cnet_split(cn, B, h8, w8, 2, ir8, df, hm, hxp, rhp, s); });
     add("coords_init", [=](cudaStream_t s) { return raft_coords_init(c0, c1p, B, h8, w8, s); });
   }

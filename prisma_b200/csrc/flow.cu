@@ -241,19 +241,26 @@ __global__ void k_pool_fmap(const __half* __restrict__ feat, size_t frame_stride
 // one fractional part, so a 10x10 neighbourhood is fetched once: lanes 10g..10g+9 (g = level group) hold one column
 // each (10 rows in registers), the right-hand column comes from lane+1 by shuffle.  Channel = l*81 + i*9 + j with
 // i moving x and j moving y (the reference's meshgrid quirk), zero outside the volume.
+// A CTA is the 8 consecutive positions i = 8 blockIdx.x .. + 7 of image blockIdx.y.  A direction whose level 0 is the
+// transpose of another's reads key k of query i at vol0[slot][k][i]: every key is one 4-byte read of its own sector, but
+// the 8 warps of the CTA read the same 32-byte sector (rows of level 0 start on sectors) while their windows overlap,
+// so it is fetched into L1 once.  At small flow the 8 windows span 10 x 17 keys: 21 sectors per query, the same as the
+// 10 rows x 40 bytes (2-3 sectors each) of a row-major read.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_corr_lookup(const float* __restrict__ v0, const float* __restrict__ v1, const float* __restrict__ v2,
-                              const float* __restrict__ v3, int B, int P, int H8, int W8, int lh0, int lw0, int lp0,
-                              int lh1, int lw1, int lp1, int lh2, int lw2, int lp2, int lh3, int lw3, int lp3,
-                              const float* __restrict__ coords, __half* __restrict__ out, int out_ld, int out_wp,
-                              int out_pad, int out_img_rows) {
-  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+struct L0Map { int slot[8]; unsigned tr; };  // FlowCorr::slot0 / tr0
+
+__global__ void __launch_bounds__(256) k_corr_lookup(const float* __restrict__ v0, const float* __restrict__ v1,
+                              const float* __restrict__ v2, const float* __restrict__ v3, L0Map m0, int P, int W8,
+                              int lh0, int lw0, int lp0, int lh1, int lw1, int lp1, int lh2, int lw2, int lp2, int lh3,
+                              int lw3, int lp3, const float* __restrict__ coords, __half* __restrict__ out, int out_ld,
+                              int out_wp, int out_pad, int out_img_rows) {
+  const int b = blockIdx.y, i = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (wid >= B * P) return;
-  const int b = wid / P, i = wid - b * P;
+  if (i >= P) return;
+  const size_t wid = (size_t)b * P + i;
   // destination row: dense (b*P + i) or a zero-bordered image (the A operand layout of the motion encoder)
   const size_t orow = out_wp > 0 ? (size_t)b * out_img_rows + (size_t)(i / W8 + out_pad) * out_wp + (i % W8) + out_pad
-                                 : (size_t)wid;
+                                 : wid;
   const float cx = coords[((size_t)b * 2 + 0) * P + i], cy = coords[((size_t)b * 2 + 1) * P + i];
   const int grp = lane / 10, col = lane - grp * 10;  // lanes 30,31 idle
 #pragma unroll
@@ -269,12 +276,16 @@ __global__ void k_corr_lookup(const float* __restrict__ v0, const float* __restr
     const float xf = floorf(x), yf = floorf(y);
     const float wx1 = x - xf, wy1 = y - yf, wx0 = 1.f - wx1, wy0 = 1.f - wy1;
     const int x0 = (int)xf - 4 + col, y0 = (int)yf - 4;
-    const float* row = vol + (size_t)wid * lp;
+    // key k of this query: row[k * ks]
+    const bool tr = lvl == 0 && ((m0.tr >> b) & 1u);
+    const float* row = lvl != 0 ? vol + wid * lp
+                                : (tr ? vol + (size_t)m0.slot[b] * P * lp + i : vol + ((size_t)m0.slot[b] * P + i) * lp);
+    const size_t ks = tr ? (size_t)lp : 1;
     float v[10];
 #pragma unroll
     for (int r = 0; r < 10; ++r) {
       const int yy = y0 + r;
-      v[r] = (active && x0 >= 0 && x0 < lw && yy >= 0 && yy < lh) ? __ldg(row + (size_t)yy * lw + x0) : 0.f;
+      v[r] = (active && x0 >= 0 && x0 < lw && yy >= 0 && yy < lh) ? __ldg(row + (size_t)(yy * lw + x0) * ks) : 0.f;
     }
     float vn[10];
 #pragma unroll
@@ -326,8 +337,8 @@ int FlowCorr::init(int dev, int batch, int h8, int w8, int n_frames, const int* 
   PRISMA_TRY(fc_alloc(allocs, &feat, (size_t)NF * rows_pad * C));
   // Levels 1..3 share one operand buffer and one volume: the pooled features of a frame are the rows [coff[l], coff[l] + ln[l])
   // of a [n123][C] matrix, so ONE GEMM per direction writes the three coarse levels side by side into rows of pitch
-  // pitch123 (level l = columns coff[l]...).  Two launches per direction instead of four: the coarse levels used to run
-  // at 2.8-3.7 TB/s against level 0's 5.1 (short launches, 8-wave ramp each).
+  // pitch123 (level l = columns coff[l]...).  Two launches per direction instead of four: short launches of the coarse
+  // levels alone ran well below level 0's store rate (8-wave ramp each).
   coff[0] = 0;
   for (int l = 0; l < 4; ++l) {
     lh[l] = H8 >> l; lw[l] = W8 >> l; ln[l] = lh[l] * lw[l];
@@ -336,10 +347,18 @@ int FlowCorr::init(int dev, int batch, int h8, int w8, int n_frames, const int* 
   n123 = coff[3] + ln[3];
   pitch123 = round_up(n123, 4);
   rows123_pad = round_up(pitch123, 256);
-  lpitch[0] = round_up(ln[0], 4);
+  lpitch[0] = round_up(ln[0], 8);  // level-0 rows start on 32-byte sectors (the transposed lookup's sharing unit)
   lrows_pad[0] = rows_pad;
+  // level 0 once per symmetric pair of directions (see init's declaration)
+  n0 = 0; tr0 = 0;
+  for (int b = 0; b < B; ++b) {
+    slot0[b] = -1;
+    for (int a = 0; a < b && slot0[b] < 0; ++a)
+      if (!((tr0 >> a) & 1u) && f1[a] == f2[b] && f2[a] == f1[b] && f1[b] != f2[b]) { slot0[b] = slot0[a]; tr0 |= 1u << b; }
+    if (slot0[b] < 0) slot0[b] = n0++;
+  }
   PRISMA_TRY(fc_alloc(allocs, &pool123, (size_t)NF * rows123_pad * C));
-  PRISMA_TRY(fc_alloc(allocs, &vol[0], (size_t)B * P * lpitch[0]));
+  PRISMA_TRY(fc_alloc(allocs, &vol[0], (size_t)n0 * P * lpitch[0]));
   PRISMA_TRY(fc_alloc(allocs, &vol123, (size_t)B * P * pitch123));
   for (int l = 1; l < 4; ++l) {
     lpitch[l] = pitch123;
@@ -354,42 +373,58 @@ int FlowCorr::init(int dev, int batch, int h8, int w8, int n_frames, const int* 
   bytes_build = flops_build = 0;
   for (int b = 0; b < B; ++b)
     for (int part = 0; part < 2; ++part) {  // part 0: level 0 against the features; part 1: levels 1..3 against the pooled rows
+      if (part == 0 && ((tr0 >> b) & 1u)) continue;
       const int ncols = part == 0 ? lpitch[0] : pitch123;
       GemmEpilogue ep;
       ep.alpha = 1.0f / sqrtf((float)C);
-      ep.out_f32 = part == 0 ? vol[0] + (size_t)b * P * lpitch[0] : vol123 + (size_t)b * P * pitch123;
+      ep.out_f32 = part == 0 ? vol[0] + (size_t)slot0[b] * P * lpitch[0] : vol123 + (size_t)b * P * pitch123;
       ep.out_f32_ld = ncols;
-      // the volume is store-bound (131 KB per 128 x 256 tile against 4 K-blocks of MMA): leave through TMA bulk stores
+      // The volume is store-bound (4 K-blocks of MMA per tile): it leaves through TMA bulk stores, in 128-wide tiles.  Their
+      // 64 KB of fp32 fit the staging boxes (8 warps x 2 x 4 KB) whole, so the consumers run the next tile's MMAs while
+      // the stores drain; a 128 x 256 tile has twice that and its warps waited for their first boxes to drain before
+      // staging the rest (H100 SXM, 700 W: 1.35 -> 1.13 ms per frame pair in the clip pass).
       GemmLaunch g;
-      ep.tma_store = gemm_pick_bn(P, ncols, num_sms) >= 128;
+      const bool wide = gemm_pick_bn(P, ncols, num_sms) >= 128;
+      ep.tma_store = wide;
       const __half* w2 = part == 0 ? feat + (size_t)f2[b] * rows_pad * C : pool123 + (size_t)f2[b] * rows123_pad * C;
       PRISMA_TRY(gemm_prepare(&g, feat + (size_t)f1[b] * rows_pad * C, P, C, C, w2, part == 0 ? rows_pad : rows123_pad, P, ncols, 1,
-                              off, ep, num_sms));
+                              off, ep, num_sms, wide ? 128 : 0));
       gemms.push_back(g);
     }
-  for (int l = 0; l < 4; ++l) {
-    flops_build += (double)B * 2.0 * P * (double)ln[l] * C;
-    bytes_build += (double)B * 4.0 * P * (double)ln[l];
+  for (int l = 0; l < 4; ++l) {  // what the GEMMs compute and write: level 0 of n0 directions, levels 1..3 of all B
+    const double dirs = l == 0 ? n0 : B;
+    flops_build += dirs * 2.0 * P * (double)ln[l] * C;
+    bytes_build += dirs * 4.0 * P * (double)ln[l];
   }
   bytes_build += 2.0 * B * P * (double)C * 2.0;  // the two fp16 feature maps of every direction, read once
   return 0;
 }
 
-int FlowCorr::set_fmaps(const float* fm1, const float* fm2) {
-  PRISMA_CHECK(NF == 2 * B, "flowcorr: set_fmaps needs the default frame layout");
+int FlowCorr::init_pairs(int dev, int npairs, int h8, int w8) {
+  PRISMA_CHECK(npairs >= 1 && npairs <= 4, "flowcorr: pairs per pass must be in [1, 4]");
+  int fr1[8], fr2[8];
+  for (int p = 0; p < npairs; ++p) { fr1[2 * p] = p; fr2[2 * p] = p + 1; fr1[2 * p + 1] = p + 1; fr2[2 * p + 1] = p; }
+  return init(dev, 2 * npairs, h8, w8, npairs + 1, fr1, fr2);
+}
+
+int FlowCorr::upload_frames(int first, int count, const float* nchw) {
   PRISMA_CUDA_OK(cudaSetDevice(device));
-  std::vector<__half> h((size_t)B * rows_pad * C, __float2half_rn(0.f));
-  for (int which = 0; which < 2; ++which) {
-    const float* src = which == 0 ? fm1 : fm2;
-    std::fill(h.begin(), h.end(), __float2half_rn(0.f));
-    for (int b = 0; b < B; ++b)
-      for (int c = 0; c < C; ++c)
-        for (int p = 0; p < P; ++p)
-          h[((size_t)b * rows_pad + p) * C + c] = __float2half_rn(src[((size_t)b * C + c) * P + p]);
-    PRISMA_CUDA_OK(cudaMemcpy(feat + (size_t)which * B * rows_pad * C, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
-  }
+  std::vector<__half> h((size_t)count * rows_pad * C, __float2half_rn(0.f));
+  for (int f = 0; f < count; ++f)
+    for (int c = 0; c < C; ++c)
+      for (int p = 0; p < P; ++p)
+        h[((size_t)f * rows_pad + p) * C + c] = __float2half_rn(nchw[((size_t)f * C + c) * P + p]);
+  PRISMA_CUDA_OK(cudaMemcpy(feat + (size_t)first * rows_pad * C, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
   return 0;
 }
+
+int FlowCorr::set_fmaps(const float* fm1, const float* fm2) {
+  PRISMA_CHECK(NF == 2 * B, "flowcorr: set_fmaps needs the default frame layout");
+  PRISMA_TRY(upload_frames(0, B, fm1));
+  return upload_frames(B, B, fm2);
+}
+
+int FlowCorr::set_frames(const float* frames) { return upload_frames(0, NF, frames); }
 
 int FlowCorr::pool_frames(int first, int count, cudaStream_t s) {
   PoolGeom g;
@@ -416,10 +451,12 @@ int FlowCorr::lookup(const float* d_coords, cudaStream_t s) {
 
 int FlowCorr::lookup_to(const float* d_coords, __half* dst, int dst_ld, int dst_wp, int dst_pad, int dst_img_rows,
                         cudaStream_t s) {
-  const int warps = B * P;
-  k_corr_lookup<<<ceil_div(warps * 32, 256), 256, 0, s>>>(vol[0], vol[1], vol[2], vol[3], B, P, H8, W8, lh[0], lw[0], lpitch[0], lh[1],
-                                                          lw[1], lpitch[1], lh[2], lw[2], lpitch[2], lh[3], lw[3], lpitch[3],
-                                                          d_coords, dst, dst_ld, dst_wp, dst_pad, dst_img_rows);
+  L0Map m0;
+  for (int b = 0; b < 8; ++b) m0.slot[b] = b < B ? slot0[b] : 0;
+  m0.tr = tr0;
+  k_corr_lookup<<<dim3(ceil_div(P, 8), B), 256, 0, s>>>(vol[0], vol[1], vol[2], vol[3], m0, P, W8, lh[0], lw[0], lpitch[0], lh[1],
+                                                        lw[1], lpitch[1], lh[2], lw[2], lpitch[2], lh[3], lw[3], lpitch[3],
+                                                        d_coords, dst, dst_ld, dst_wp, dst_pad, dst_img_rows);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -462,9 +499,19 @@ int FlowCorr::lookup_host(const float* c, float* out_nchw, int iters, float* ms)
 }
 
 int FlowCorr::read_level(int level, int b, int row0, int nrows, float* out) {
-  PRISMA_CHECK(level >= 0 && level < 4 && b >= 0 && b < B && row0 >= 0 && row0 + nrows <= P, "flowcorr: bad range");
+  PRISMA_CHECK(level >= 0 && level < 4 && b >= 0 && b < B && row0 >= 0 && nrows >= 0 && row0 + nrows <= P,
+               "flowcorr: bad range");
   PRISMA_CUDA_OK(cudaSetDevice(device));
-  PRISMA_CUDA_OK(cudaMemcpy2D(out, (size_t)ln[level] * 4, vol[level] + ((size_t)b * P + row0) * lpitch[level],
+  if (level == 0 && ((tr0 >> b) & 1u)) {  // columns [row0, row0 + nrows) of the partner's volume, transposed
+    std::vector<float> t((size_t)ln[0] * nrows);
+    PRISMA_CUDA_OK(cudaMemcpy2D(t.data(), (size_t)nrows * 4, vol[0] + (size_t)slot0[b] * P * lpitch[0] + row0,
+                                (size_t)lpitch[0] * 4, (size_t)nrows * 4, ln[0], cudaMemcpyDeviceToHost));
+    for (int k = 0; k < ln[0]; ++k)
+      for (int r = 0; r < nrows; ++r) out[(size_t)r * ln[0] + k] = t[(size_t)k * nrows + r];
+    return 0;
+  }
+  const size_t row = level == 0 ? (size_t)slot0[b] * P + row0 : (size_t)b * P + row0;
+  PRISMA_CUDA_OK(cudaMemcpy2D(out, (size_t)ln[level] * 4, vol[level] + row * lpitch[level],
                               (size_t)lpitch[level] * 4, (size_t)ln[level] * 4, nrows, cudaMemcpyDeviceToHost));
   return 0;
 }
