@@ -7,6 +7,7 @@ process_image(args), process_video(args), the CLI flags of bands/depth_anything.
 (:155-166,241-251).  The model call and the numpy encode are replaced by libprisma_b200.so; there is no CPU path.
 
 `--metric indoor|outdoor` runs the ZoeDepth metric head (no flip in the encode, reference :188).
+`--ply` writes <band>.ply next to a still image's output (reference :170-171); video runs ignore it, as the reference does.
 Additions: --weights (state_dict: torch .pth/.pt or .npz), --seeded-weights (offline test weights), --device.
 """
 import argparse
@@ -20,6 +21,7 @@ from bands.common.meta import get_target, get_url, is_video, load_metadata, writ
 from bands.common.depth_loop import process_depth_video  # noqa: E402
 from bands.common.sharded import ENV_RANK, ShardContext, launch  # noqa: E402
 from bands.common.media import open_rgb, write_rgb  # noqa: E402
+from bands.common.ply import write_ply  # noqa: E402
 
 BAND = "depth_anything"
 DEVICE = 0
@@ -68,6 +70,8 @@ def process_image(a):
     rgb, dmin, dmax, pred = model.infer_image(img, want_depth=True)  # write_depth's PNG encoding (io.py:138-166)
     if a.npy:
         np.save(os.path.splitext(a.output)[0] + ".npy", pred)
+    if a.ply:  # reference :170-171: write_pcl(..., flip=flip), flip = (metric == 'none')
+        write_ply(os.path.join(os.path.dirname(a.output), BAND + ".ply"), model.point_cloud(pred, img, flip=a.metric == "none"))
     write_rgb(a.output, rgb)
     if data:
         data["bands"][BAND]["values"] = {"min": {"type": "float", "value": dmin}, "max": {"type": "float", "value": dmax}}
@@ -99,8 +103,6 @@ def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.metric != "none" and args.encoder != "vitl" and not args.seeded_weights:
         raise ValueError("the metric checkpoints are ViT-L models (base_models/depth_anything.py:339)")
-    if args.ply:
-        print("--ply is outside the engine's scope (optional export, SURVEY.md section 2); ignored")
     data = load_metadata(args.input)
     if data:
         args.input = get_url(args.input, data, "rgba")

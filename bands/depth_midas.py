@@ -7,8 +7,10 @@ depth_midas_min.csv, depth_midas_max.csv, optional <sub>/%05d.npy|png) and the m
 The hub transform, the DPT_Large forward, the bicubic(align_corners=True) resize and the heat encode run in
 libprisma_b200.so; there is no CPU path.
 
-Built: --model midas3 (the default: DPT_Large + default_transform).  midas2 / midas2-small (the ResNeXt-101 MiDaS v2.1
-network) and midas3-small (DPT_Large behind the 256-pixel small_transform) raise instead of falling back.
+Built: --model midas3 (the default: DPT_Large + default_transform, fit inside 384 x 384) and midas3-small (the same network
+and checkpoint behind the hub's small_transform, fit inside 256 x 256).  midas2 / midas2-small (the ResNeXt-101 MiDaS v2.1
+network) raise instead of falling back.  --ply writes depth_midas.ply next to a still image's output (reference :102-103);
+video runs ignore it, as the reference does.
 Additions: --weights (the upstream dpt_large_384.pt state_dict or .npz), --seeded-weights, --device.
 """
 import argparse
@@ -21,6 +23,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from bands.common.depth_loop import process_depth_video  # noqa: E402
 from bands.common.sharded import ENV_RANK, ShardContext, launch  # noqa: E402
 from bands.common.media import open_rgb, write_rgb  # noqa: E402
+from bands.common.ply import write_ply  # noqa: E402
 from bands.common.meta import get_target, get_url, is_video, load_metadata, write_metadata  # noqa: E402
 
 BAND = "depth_midas"
@@ -45,13 +48,16 @@ def _load_state_dict(a):
     return sd.get("state_dict", sd)
 
 
+NET_SIDES = {"midas3": 384, "midas3-small": 256}  # hub default_transform / small_transform
+
+
 def init_model(model_version="midas3"):
     """reference :29-46."""
     global model
-    if model_version != "midas3":
-        raise NotImplementedError("only --model midas3 (DPT_Large, default transform) is built; %s is not" % model_version)
+    if model_version not in NET_SIDES:
+        raise NotImplementedError("only --model midas3 / midas3-small (DPT_Large) are built; %s is not" % model_version)
     from prisma_b200.depth import MidasEngine
-    model = MidasEngine(_load_state_dict(args), device=args.device if args else DEVICE)
+    model = MidasEngine(_load_state_dict(args), device=args.device if args else DEVICE, net_side=NET_SIDES[model_version])
     return model
 
 
@@ -67,6 +73,8 @@ def process_image(a):
     rgb, dmin, dmax, pred = model.infer_image(img, want_depth=True)  # write_depth's PNG encoding (io.py:138-166)
     if a.npy:
         np.save(os.path.join(os.path.dirname(a.output), BAND + ".npy"), pred)
+    if a.ply:  # reference :102-103: write_pcl(..., flip=True)
+        write_ply(os.path.join(os.path.dirname(a.output), BAND + ".ply"), model.point_cloud(pred, img, flip=True))
     write_rgb(a.output, rgb)
     if data:
         data["bands"][BAND]["values"] = {"min": {"value": dmin, "type": "float"}, "max": {"value": dmax, "type": "float"}}
@@ -95,8 +103,6 @@ def build_parser():
 def main(argv=None):
     global args, data
     args = build_parser().parse_args(argv)
-    if args.ply:
-        print("--ply is outside the engine's scope (optional export, SURVEY.md section 2); ignored")
     data = load_metadata(args.input)
     if data:
         args.input = get_url(args.input, data, "rgba")

@@ -67,6 +67,15 @@ int prisma_depth_infer_image(prisma_engine* e, const uint8_t* rgb, int h, int w,
                              float* min_out, float* max_out);
 int prisma_depth_encode_png(prisma_engine* e, const float* prediction, int h, int w, int flip, uint8_t* rgb_out,
                             float* min_out, float* max_out);
+/* --ply of a still image = write_pcl (bands/common/io.py:201-211, common/geom.py:5-47) of an h*w f32 prediction:
+ * flip != 0 first maps d -> min + (1 - (d - min)/(max - min)) * (max - min) in f32, then cv2.medianBlur(d, 5)
+ * (BORDER_REPLICATE) and the unprojection with u0 = w/2, v0 = h/2, fx = fy = 1000.  rgb: the h*w*3 u8 RGB frame.
+ * out_records: h*w 15-byte little-endian vertex records (x, y, z f32; red, green, blue u8), row-major, bit-exact.   */
+int prisma_depth_point_cloud(prisma_engine* e, const float* prediction, int h, int w, int flip, const uint8_t* rgb,
+                             uint8_t* out_records);
+/* MiDaS engines ("dpt_large", "dpt_tiny") only, before the first frame: the side of the transform's fit-inside box,
+ * 384 (hubconf default_transform, midas3) or 256 (small_transform, midas3-small).                               */
+int prisma_depth_set_net_side(prisma_engine* e, int side);
 /* Intermediate tensors of the last prisma_depth_infer call as dense fp32 (tests only):
  * "net_input" [3][hn][wn], "tokens" [T][D], "feat0".."feat3" [T][D], "net_depth" [hn][wn], ...
  * returns the number of floats written, or negative.                                                       */

@@ -54,6 +54,8 @@ SIGNATURES = {
     "prisma_depth_encode": (C.c_int, [C.c_void_p, c_float_p, C.c_int, C.c_int, C.c_int, c_u8_p, c_float_p, c_float_p]),
     "prisma_depth_encode_png": (C.c_int, [C.c_void_p, c_float_p, C.c_int, C.c_int, C.c_int, c_u8_p, c_float_p, c_float_p]),
     "prisma_depth_infer_image": (C.c_int, [C.c_void_p, c_u8_p, C.c_int, C.c_int, c_float_p, c_u8_p, c_float_p, c_float_p]),
+    "prisma_depth_point_cloud": (C.c_int, [C.c_void_p, c_float_p, C.c_int, C.c_int, C.c_int, c_u8_p, c_u8_p]),
+    "prisma_depth_set_net_side": (C.c_int, [C.c_void_p, C.c_int]),
     "prisma_depth_read_tap": (C.c_longlong, [C.c_void_p, C.c_char_p, c_float_p, C.c_longlong]),
     "prisma_depth_profile": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_float_p]),
     "prisma_depth_work": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_double_p]),

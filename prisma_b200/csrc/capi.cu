@@ -189,6 +189,20 @@ int prisma_depth_infer_image(prisma_engine* e, const uint8_t* rgb, int h, int w,
   return d ? d->infer_image(rgb, h, w, depth_out, png_rgb_out, min_out, max_out) : -1;
   API_GUARD_END
 }
+int prisma_depth_point_cloud(prisma_engine* e, const float* prediction, int h, int w, int flip, const uint8_t* rgb,
+                             uint8_t* out_records) {
+  API_GUARD_BEGIN
+  DepthEngine* d = as_depth(e);
+  PRISMA_CHECK(prediction && rgb && out_records, "null argument");
+  return d ? d->point_cloud(prediction, h, w, flip, rgb, out_records) : -1;
+  API_GUARD_END
+}
+int prisma_depth_set_net_side(prisma_engine* e, int side) {
+  API_GUARD_BEGIN
+  DepthEngine* d = as_depth(e);
+  return d ? d->set_net_side(side) : -1;
+  API_GUARD_END
+}
 long long prisma_depth_read_tap(prisma_engine* e, const char* name, float* out, long long capacity) {
   API_GUARD_BEGIN
   DepthEngine* d = as_depth(e);

@@ -47,13 +47,14 @@ void da_net_size(int W, int H, int* wn, int* hn) {
 
 // MiDaS transform = hubconf default_transform, which bands/depth_midas.py:37-40 selects for DPT_Large: the Resize class
 // vendored in d_anything/util/transform.py (get_size :111-166, constrain_to_multiple_of :98-109) with
-// resize_method="upper_bound", keep_aspect_ratio, multiple of 32, target 384 x 384: the frame is scaled to FIT 384 x 384.
-void midas_net_size(int W, int H, int* wn, int* hn) {
-  double sh = 384.0 / H, sw = 384.0 / W;
+// resize_method="upper_bound", keep_aspect_ratio, multiple of 32, target side x side: the frame is scaled to FIT it.
+// side 384 is that default_transform; side 256 is the hub's small_transform (midas3-small), otherwise identical.
+void midas_net_size(int W, int H, int* wn, int* hn, int side) {
+  double sh = (double)side / H, sw = (double)side / W;
   if (sw < sh) sh = sw; else sw = sh;
-  auto constrain = [](double x) {
+  auto constrain = [side](double x) {
     int y = (int)(nearbyint(x / 32.0) * 32.0);   // np.round: half to even, as nearbyint
-    if (y > 384) y = (int)(floor(x / 32.0) * 32.0);
+    if (y > side) y = (int)(floor(x / 32.0) * 32.0);
     return y;
   };
   *hn = constrain(sh * H);
@@ -397,7 +398,7 @@ int DepthEngine::build_plan(int H, int W, int Bt) {
   plan_H = plan_W = 0;
 
   const bool midas = family == FAMILY_MIDAS;
-  if (midas) midas_net_size(W, H, &wn, &hn);
+  if (midas) midas_net_size(W, H, &wn, &hn, net_side);
   else if (metric) { hn = 392; wn = 518; }  // config_zoedepth.json img_size, keep_aspect_ratio False (PrepForMidas)
   else da_net_size(W, H, &wn, &hn);
   PRISMA_CHECK(hn >= patch * 2 && wn >= patch * 2, "frame too small for the network input");
@@ -956,6 +957,36 @@ int DepthEngine::encode(const float* pred, int H, int W, int flip, uint8_t* rgb_
   if (min_out) *min_out = mm[0];
   if (max_out) *max_out = mm[1];
   return r;
+}
+
+int DepthEngine::point_cloud(const float* pred, int H, int W, int flip, const uint8_t* rgb, uint8_t* records_out) {
+  PRISMA_CHECK(H > 0 && W > 0, "point cloud: bad frame size");
+  PRISMA_CUDA_OK(cudaSetDevice(device));
+  const size_t n = (size_t)H * W;
+  float* d_pred = nullptr; float* d_med = nullptr; uint8_t* d_rgb = nullptr; uint8_t* d_rec = nullptr; uint32_t* d_mm = nullptr;
+  std::vector<void*> tmp;
+  auto cleanup = [&]() { for (void* q : tmp) cudaFree(q); };
+  int r = 0;
+  if ((r = dev_alloc(tmp, &d_pred, n, false)) || (r = dev_alloc(tmp, &d_med, n, false)) || (r = dev_alloc(tmp, &d_rgb, n * 3, false)) ||
+      (r = dev_alloc(tmp, &d_rec, n * 15, false)) || (r = dev_alloc(tmp, &d_mm, 2))) { cleanup(); return r; }
+  cudaMemcpyAsync(d_pred, pred, n * 4, cudaMemcpyHostToDevice, stream);
+  cudaMemcpyAsync(d_rgb, rgb, n * 3, cudaMemcpyHostToDevice, stream);
+  r = depth_point_cloud(d_pred, H, W, flip ? 1 : 0, d_rgb, d_med, d_rec, d_mm, num_sms, stream);
+  if (r == 0) {
+    cudaMemcpyAsync(records_out, d_rec, n * 15, cudaMemcpyDeviceToHost, stream);
+    cudaError_t e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) { set_last_error(std::string("point_cloud: ") + cudaGetErrorString(e)); r = -2; }
+  }
+  cleanup();
+  return r;
+}
+
+int DepthEngine::set_net_side(int side) {
+  PRISMA_CHECK(family == FAMILY_MIDAS, "the network input side is a MiDaS transform setting");
+  PRISMA_CHECK(side == 384 || side == 256, "MiDaS transform side must be 384 (default) or 256 (small)");
+  PRISMA_CHECK(plan_H == 0 && plan_W == 0, "set the MiDaS transform side before the first frame");
+  net_side = side;
+  return 0;
 }
 
 long long DepthEngine::read_tap(const std::string& name, float* out, long long capacity) {

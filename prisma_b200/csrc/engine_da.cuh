@@ -45,7 +45,7 @@ struct Step { int group; const char* name; std::function<int(cudaStream_t)> fn; 
 struct PMap;
 
 void da_net_size(int W, int H, int* wn, int* hn);
-void midas_net_size(int W, int H, int* wn, int* hn);
+void midas_net_size(int W, int H, int* wn, int* hn, int side = 384);
 enum DepthFamily { FAMILY_DA = 0, FAMILY_MIDAS = 1 };
 
 class DepthEngine {
@@ -58,6 +58,8 @@ class DepthEngine {
   int infer_resident(int H, int W, int n, int iters, float* ms_per_iter);
   int encode(const float* pred, int H, int W, int flip, uint8_t* rgb_out, float* min_out, float* max_out, int png_variant = 0);
   int infer_image(const uint8_t* rgb, int H, int W, float* depth_out, uint8_t* png_rgb_out, float* min_out, float* max_out);
+  int point_cloud(const float* pred, int H, int W, int flip, const uint8_t* rgb, uint8_t* records_out);
+  int set_net_side(int side);
   long long read_tap(const std::string& name, float* out, long long capacity);
   int profile(int H, int W, int n, float* out8);
   int build_plan(int H, int W, int batch);
@@ -91,6 +93,7 @@ class DepthEngine {
   int D = 0, depth = 0, heads = 0, F = 0, oc[4] = {0, 0, 0, 0};
   // family switches: Depth-Anything (DINOv2 ViT/14 + DPT head) or MiDaS DPT (timm ViT/16, "project" readout, hooks)
   int family = FAMILY_DA, patch = 14, pos_grid = 37, hooks[4] = {0, 0, 0, 0};
+  int net_side = 384;  // MiDaS transform side: 384 (hub default_transform) or 256 (small_transform)
   float* zoe_metric = nullptr; float* zoe_tmp = nullptr; int plan_W_req = 0;
   bool metric = false;  // --metric indoor|outdoor: ZoeDepth head on the relative model, fixed 392 x 518 network input
   std::vector<float> host_pos, host_cls;  // MiDaS: pos-embed resized on the host per resolution (bilinear)

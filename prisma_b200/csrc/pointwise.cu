@@ -481,6 +481,134 @@ int depth_encode_png(const float* pred, int H, int W, int flip, uint8_t* rgb_out
 }
 
 // ------------------------------------------------------------------------------------------------
+// Point cloud of a still image = write_pcl (bands/common/io.py:201-211) -> create_point_cloud (common/geom.py:5-24):
+//   (a) flip (only when asked): t = (d-min)/(max-min); t = 1-t; d = min + t*(max-min), all f32
+//   (b) cv2.medianBlur(d, 5): the 13th of the 25 values of the 5x5 window, BORDER_REPLICATE
+//   (c) X = d*((x-W/2)/1000), Y = d*(-((y-H/2)/1000)), Z = d*(-1), f32 -> 15-byte records x y z f4, red green blue u1
+// Every f32 operation is rounded separately (__f*_rn), as numpy does, so no FMA contraction can change a bit.
+// Per pixel: the median reads 4 B (+ the halo, from shared memory) and writes 4 B; the pack reads 4 + 3 B and writes 15 B.
+// ------------------------------------------------------------------------------------------------
+constexpr int PCL_TILE = 32, PCL_THREADS_Y = 8, PCL_HALO = 2;
+constexpr int PCL_SPAN = PCL_TILE + 2 * PCL_HALO;
+
+__device__ __forceinline__ float pcl_flip(float d, float dmin, float range) {
+  const float t = __fsub_rn(1.0f, __fdiv_rn(__fsub_rn(d, dmin), range));
+  return __fadd_rn(dmin, __fmul_rn(t, range));
+}
+
+// Median of 25: Batcher's odd-even merge sort for 32 inputs, with the comparators that touch inputs 25..31 dropped (padding
+// with +inf never moves) and only those that feed position 12 kept: 113 compare-exchanges.  The median of a 5x5 window is a
+// value of the window whatever the ties, so any correct selection network gives the reference's bits.
+__device__ __forceinline__ float median25(float* v) {
+#define CE(i, j) { const float a = v[i], b = v[j]; v[i] = fminf(a, b); v[j] = fmaxf(a, b); }
+  CE(0,1) CE(2,3) CE(4,5) CE(6,7) CE(8,9) CE(10,11) CE(12,13) CE(14,15) CE(16,17) CE(18,19) CE(20,21) CE(22,23)
+  CE(0,2) CE(1,3) CE(4,6) CE(5,7) CE(8,10) CE(9,11) CE(12,14) CE(13,15) CE(16,18) CE(17,19) CE(20,22) CE(21,23)
+  CE(1,2) CE(5,6) CE(9,10) CE(13,14) CE(17,18) CE(21,22) CE(0,4) CE(1,5) CE(2,6) CE(3,7) CE(8,12) CE(9,13) CE(10,14)
+  CE(11,15) CE(16,20) CE(17,21) CE(18,22) CE(19,23) CE(2,4) CE(3,5) CE(10,12) CE(11,13) CE(18,20) CE(19,21) CE(1,2)
+  CE(3,4) CE(5,6) CE(9,10) CE(11,12) CE(13,14) CE(17,18) CE(19,20) CE(21,22) CE(0,8) CE(1,9) CE(2,10) CE(3,11)
+  CE(4,12) CE(5,13) CE(6,14) CE(7,15) CE(16,24) CE(4,8) CE(5,9) CE(6,10) CE(7,11) CE(20,24) CE(2,4) CE(3,5) CE(6,8)
+  CE(7,9) CE(10,12) CE(11,13) CE(18,20) CE(19,21) CE(22,24) CE(1,2) CE(3,4) CE(5,6) CE(7,8) CE(9,10) CE(11,12)
+  CE(13,14) CE(17,18) CE(19,20) CE(21,22) CE(23,24) CE(0,16) CE(1,17) CE(2,18) CE(3,19) CE(4,20) CE(5,21) CE(6,22)
+  CE(7,23) CE(8,24) CE(8,16) CE(9,17) CE(10,18) CE(11,19) CE(12,20) CE(13,21) CE(6,10) CE(7,11) CE(12,16) CE(13,17)
+  CE(10,12) CE(11,13) CE(11,12)
+#undef CE
+  return v[12];
+}
+
+// One 32 x 32 output tile per block of 32 x 8 threads: the 36 x 36 input window (replicated borders, flipped on load) is
+// staged once in shared memory; each thread selects four medians in registers.
+__global__ void __launch_bounds__(PCL_TILE * PCL_THREADS_Y) k_pcl_median5(const float* __restrict__ d, int H, int W,
+                                                                          const uint32_t* __restrict__ mm, int flip,
+                                                                          float* __restrict__ out) {
+  __shared__ float t[PCL_SPAN][PCL_SPAN];
+  const int x0 = blockIdx.x * PCL_TILE, y0 = blockIdx.y * PCL_TILE;
+  float dmin = 0.f, range = 0.f;
+  if (flip) { dmin = ord2f(mm[0]); range = __fsub_rn(ord2f(mm[1]), dmin); }
+  const int tid = threadIdx.y * PCL_TILE + threadIdx.x;
+  for (int i = tid; i < PCL_SPAN * PCL_SPAN; i += PCL_TILE * PCL_THREADS_Y) {
+    const int r = i / PCL_SPAN, c = i - r * PCL_SPAN;
+    const int gy = min(max(y0 + r - PCL_HALO, 0), H - 1), gx = min(max(x0 + c - PCL_HALO, 0), W - 1);
+    const float v = d[(size_t)gy * W + gx];
+    t[r][c] = flip ? pcl_flip(v, dmin, range) : v;
+  }
+  __syncthreads();
+  const int x = x0 + threadIdx.x;
+#pragma unroll
+  for (int k = 0; k < PCL_TILE / PCL_THREADS_Y; ++k) {
+    const int ry = threadIdx.y + k * PCL_THREADS_Y, y = y0 + ry;
+    float v[25];
+#pragma unroll
+    for (int dy = 0; dy < 5; ++dy)
+#pragma unroll
+      for (int dx = 0; dx < 5; ++dx) v[dy * 5 + dx] = t[ry + dy][threadIdx.x + dx];
+    const float m = median25(v);
+    if (x < W && y < H) out[(size_t)y * W + x] = m;
+  }
+}
+
+// 256 pixels per block: the block's 768 colour bytes are staged in shared memory, each thread assembles its 15-byte record
+// there, and the block writes its 3840 contiguous record bytes as 16-byte stores (3840 = 240 * 16, so every full block
+// starts 16-byte aligned).
+constexpr int PCL_PACK = 256;
+__global__ void __launch_bounds__(PCL_PACK) k_pcl_unproject_pack(const float* __restrict__ d, const uint8_t* __restrict__ rgb,
+                                                                 int H, int W, uint8_t* __restrict__ out) {
+  __shared__ __align__(16) uint8_t col[PCL_PACK * 3];
+  __shared__ __align__(16) uint8_t rec[PCL_PACK * 15];
+  const long long n = (long long)H * W, p0 = (long long)blockIdx.x * PCL_PACK;
+  const int cnt = (int)min((long long)PCL_PACK, n - p0);
+  const uint8_t* src = rgb + p0 * 3;
+  uint8_t* dst = out + p0 * 15;
+  if (cnt == PCL_PACK) {
+    for (int i = threadIdx.x; i < PCL_PACK * 3 / 16; i += PCL_PACK)
+      reinterpret_cast<uint4*>(col)[i] = reinterpret_cast<const uint4*>(src)[i];
+  } else {
+    for (int i = threadIdx.x; i < cnt * 3; i += PCL_PACK) col[i] = src[i];
+  }
+  __syncthreads();
+  if (threadIdx.x < cnt) {
+    const long long p = p0 + threadIdx.x;
+    const int y = (int)(p / W), x = (int)(p - (long long)y * W);
+    const float dv = d[p];
+    const float u0 = 0.5f * (float)W, v0 = 0.5f * (float)H;  // rgb.shape[1] / 2, rgb.shape[0] / 2: exact in f32
+    const float xyz[3] = {__fmul_rn(dv, __fdiv_rn(__fsub_rn((float)x, u0), 1000.0f)),
+                          __fmul_rn(dv, -__fdiv_rn(__fsub_rn((float)y, v0), 1000.0f)),
+                          __fmul_rn(dv, -1.0f)};
+    uint8_t* o = rec + threadIdx.x * 15;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const uint32_t b = __float_as_uint(xyz[c]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) o[c * 4 + k] = (uint8_t)(b >> (8 * k));
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[12 + c] = col[threadIdx.x * 3 + c];
+  }
+  __syncthreads();
+  if (cnt == PCL_PACK) {
+    for (int i = threadIdx.x; i < PCL_PACK * 15 / 16; i += PCL_PACK)
+      reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(rec)[i];
+  } else {
+    for (int i = threadIdx.x; i < cnt * 15; i += PCL_PACK) dst[i] = rec[i];
+  }
+}
+
+int depth_point_cloud(const float* depth, int H, int W, int flip, const uint8_t* rgb, float* blurred, uint8_t* records,
+                      uint32_t* mm_scratch, int num_sms, cudaStream_t s) {
+  PRISMA_CHECK(H > 0 && W > 0, "point cloud: empty frame");
+  PRISMA_CHECK(H <= 65535 * PCL_TILE, "point cloud: frame too tall");
+  const long long n = (long long)H * W;
+  if (flip) {
+    k_minmax_init<<<1, 1, 0, s>>>(mm_scratch);
+    k_minmax_plain<<<num_sms * 4, 256, 0, s>>>(depth, n, mm_scratch);
+  }
+  k_pcl_median5<<<dim3((W + PCL_TILE - 1) / PCL_TILE, (H + PCL_TILE - 1) / PCL_TILE), dim3(PCL_TILE, PCL_THREADS_Y), 0, s>>>(
+      depth, H, W, mm_scratch, flip, blurred);
+  k_pcl_unproject_pack<<<(unsigned)((n + PCL_PACK - 1) / PCL_PACK), PCL_PACK, 0, s>>>(blurred, rgb, H, W, records);
+  PRISMA_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // small utilities
 // ------------------------------------------------------------------------------------------------
 __global__ void k_f32_to_f16(const float* __restrict__ a, __half* __restrict__ b, long long n) {

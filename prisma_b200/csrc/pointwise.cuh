@@ -20,6 +20,10 @@ int depth_encode_only(const float* pred, int H, int W, int flip, uint8_t* rgb_ou
                       float* minmax_out, int num_sms, cudaStream_t s);
 int depth_encode_png(const float* pred, int H, int W, int flip, uint8_t* rgb_out, uint32_t* mm_scratch,
                      unsigned long long* mag_scratch, float* minmax_out, int num_sms, cudaStream_t s);
+// write_pcl's point cloud of an H x W prediction: optional flip, 5x5 median (-> blurred, H*W f32), unprojection packed
+// with the u8 RGB frame into H*W 15-byte records (x, y, z f32, red, green, blue u8)
+int depth_point_cloud(const float* depth, int H, int W, int flip, const uint8_t* rgb, float* blurred, uint8_t* records,
+                      uint32_t* mm_scratch, int num_sms, cudaStream_t s);
 int readout_concat_f16(const float* x, int batch, int T, int D, __half* out, cudaStream_t s);
 int upsample_bicubic_ac_f32(const float* in, int ih, int iw, float* out, int oh, int ow, int num_sms, cudaStream_t s);
 int f32_to_f16(const float* a, __half* b, long long n, cudaStream_t s);

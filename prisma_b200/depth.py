@@ -8,7 +8,10 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import PrismaError, check, fptr, lib, u8ptr, c_i64_p
+from ._lib import PrismaError, check, fptr, lib, u8ptr, c_i64_p, c_u8_p
+
+# save_point_cloud's vertex dtype (bands/common/geom.py:31-32): 15-byte packed little-endian records
+PLY_VERTEX_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"), ("blue", "u1")])
 
 
 def da_net_size(width, height):
@@ -159,6 +162,19 @@ class DepthAnythingEngine:
         check(lib().prisma_depth_infer_image(self._h, u8ptr(img), h, w, fptr(pred), u8ptr(rgb), C.byref(dmin), C.byref(dmax)))
         return rgb, dmin.value, dmax.value, pred
 
+    def point_cloud(self, pred, rgb, flip):
+        """write_pcl (bands/common/io.py:201-211) of an HxW f32 prediction and its HxWx3 u8 RGB frame: the H*W vertices
+        save_point_cloud writes, as a structured array of PLY_VERTEX_DTYPE (optional flip, 5x5 median, unprojection)."""
+        p = np.ascontiguousarray(pred, dtype=np.float32)
+        img = np.ascontiguousarray(rgb)
+        if p.ndim != 2 or img.dtype != np.uint8 or img.shape != p.shape + (3,):
+            raise PrismaError("expected an HxW prediction and an HxWx3 uint8 RGB frame of the same size")
+        h, w = p.shape
+        out = np.empty(h * w, PLY_VERTEX_DTYPE)
+        check(lib().prisma_depth_point_cloud(self._h, fptr(p), h, w, int(bool(flip)), u8ptr(img),
+                                             out.ctypes.data_as(c_u8_p)))
+        return out
+
     def read_tap(self, name, shape):
         out = np.empty(int(np.prod(shape)), np.float32)
         n = check(lib().prisma_depth_read_tap(self._h, name.encode(), fptr(out), out.size))
@@ -197,10 +213,14 @@ class DepthAnythingEngine:
 class MidasEngine(DepthAnythingEngine):
     """depth_midas band (bands/depth_midas.py): MiDaS v3 DPT_Large on the same engine -- timm ViT-L/16 encoder with the
     "project" readout at blocks 5/11/17/23, the DPT RefineNet head, bicubic(align_corners=True) to the frame size.
-    `state_dict` is the upstream DPTDepthModel checkpoint (dpt_large_384.pt) as is."""
+    `state_dict` is the upstream DPTDepthModel checkpoint (dpt_large_384.pt) as is.  `net_side` is the side of the
+    transform's fit-inside box: 384 (the hub's default_transform, midas3) or 256 (small_transform, midas3-small)."""
 
-    def __init__(self, state_dict=None, device=0, variant="dpt_large"):
-        super().__init__(variant, state_dict, device)
+    def __init__(self, state_dict=None, device=0, variant="dpt_large", net_side=384):
+        super().__init__(variant, None, device)
+        check(lib().prisma_depth_set_net_side(self._h, int(net_side)))
+        if state_dict is not None:
+            self.load_state_dict(state_dict)
 
 
 class ZoeDepthEngine(DepthAnythingEngine):
