@@ -311,6 +311,34 @@ int prisma_debug_upsample_ac(int device, const float* in, int B, int ih, int iw,
 int prisma_debug_upsample_bicubic(int device, const float* in, int ih, int iw, float* out, int oh, int ow);
 /* OpenCV-exact cubic resize + normalise (K1): rgb u8 h*w*3 -> f32 [3][hn][wn]                                */
 int prisma_debug_da_preprocess(int device, const uint8_t* rgb, int h, int w, float* out, int hn, int wn);
+/* RAFT kernels, one launch each, on host buffers.  Maps use the engine's shared-border layout: pixel (y, x) of image b at row
+ * b * img_rows + y (W + pad) + x, img_rows = round_up((H + pad)(W + pad), 32); fp16 values are returned as fp32, and every
+ * destination is filled with all-ones bytes (NaN) before the launch and returned whole.  Coordinates are [B][2][H][W].    */
+/* stem im2col: x [B][3][H][W] -> out [B*(H/2)*(W/2)][192], k = (c*7 + ky)*8 + kx (kx = 7 and k >= 168 zero)               */
+int prisma_debug_raft_stem_im2col(int device, const float* x, int B, int H, int W, float* out);
+/* InstanceNorm statistics of a dense x [B][HW][C] (two-stage path) -> stats [B][C][2] = (mean, 1/sqrt(var + 1e-5))      */
+int prisma_debug_instnorm_stats(int device, const float* x, int B, int HW, int C, float* stats);
+/* the same from per-slab partial sums part [B*spi][2][C] (sum, sum of squares), normalising over HW pixels               */
+int prisma_debug_instnorm_slab_stats(int device, const float* part, int B, int spi, int C, int HW, float* stats);
+/* out = relu(skip + relu((x - mean) rstd)) into a pad-1 map out [B*img_rows][C]; x [B][H][W][C], stats [B][C][2];
+ * skip_kind 0: no skip; 1: skip [B][H][W][C] rounded to fp16 in a pad-1 map; 2: raw fp32 skip [B][H][W][C] normalised
+ * with skip_stats [B][C][2]                                                                                              */
+int prisma_debug_instnorm_apply(int device, const float* x, const float* stats, int B, int H, int W, int C, int skip_kind,
+                                const float* skip, const float* skip_stats, float* out);
+/* cnet split, then the flow columns, into the pad-2 GRU operand maps: cn [F][H*W][256] (direction b reads frame
+ * dir_frames[b]) -> h_master [B*img_rows][128], hx and rhx [B*img_rows][384]                                             */
+int prisma_debug_raft_gru_operands(int device, const float* cn, int F, int B, int H, int W, const int* dir_frames,
+                                   const float* c0, const float* c1, float* h_master, float* hx, float* rhx);
+/* convf1 im2col of the flow c1 - c0 -> out [B*H*W][256] = [98 hi | 30 zero | 98 lo | 30 zero]                            */
+int prisma_debug_raft_flow_im2col(int device, const float* c0, const float* c1, int B, int H, int W, float* out);
+/* FlowHead.conv2 gather: coords1_out = coords1_in + (b0, b1) + sum_t u_t(p + t); u [B][H][W][32] (column t*2 + o) is
+ * placed in a pad-2 map whose pad and tail rows are zero                                                                 */
+int prisma_debug_raft_flow_head2(int device, const float* u, int B, int H, int W, float b0, float b1, const float* coords1_in,
+                                 float* coords1_out);
+/* convex up-sampling of the flow c1 - c0 with mask [B][H][W][576] (in a pad-2 map), cropped: out [B][Hs][Ws][2] holds up-sampled
+ * pixel (Y + pad_top, X + pad_left)                                                                                      */
+int prisma_debug_raft_convex_upsample(int device, const float* mask, const float* c0, const float* c1, int B, int H, int W,
+                                      int Hs, int Ws, int pad_top, int pad_left, float* out);
 
 #ifdef __cplusplus
 }

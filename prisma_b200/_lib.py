@@ -119,6 +119,18 @@ SIGNATURES = {
                                            c_float_p, c_float_p]),
     "prisma_debug_upsample_bicubic": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, c_float_p, C.c_int, C.c_int]),
     "prisma_debug_da_preprocess": (C.c_int, [C.c_int, c_u8_p, C.c_int, C.c_int, c_float_p, C.c_int, C.c_int]),
+    "prisma_debug_raft_stem_im2col": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_instnorm_stats": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_instnorm_slab_stats": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_instnorm_apply": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                              c_float_p, c_float_p, c_float_p]),
+    "prisma_debug_raft_gru_operands": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                                 c_float_p, c_float_p, c_float_p, c_float_p, c_float_p]),
+    "prisma_debug_raft_flow_im2col": (C.c_int, [C.c_int, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p]),
+    "prisma_debug_raft_flow_head2": (C.c_int, [C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, c_float_p,
+                                               c_float_p]),
+    "prisma_debug_raft_convex_upsample": (C.c_int, [C.c_int, c_float_p, c_float_p, c_float_p, C.c_int, C.c_int, C.c_int,
+                                                    C.c_int, C.c_int, C.c_int, C.c_int, c_float_p]),
 }
 
 

@@ -76,6 +76,25 @@ int timed(cudaStream_t s, int iters, float* ms_out, const std::function<int()>& 
   cudaEventDestroy(b);
   return 0;
 }
+int f16_to_host(const __half* d, size_t n, float* out) {
+  std::vector<__half> h(n);
+  PRISMA_CUDA_OK(cudaMemcpy(h.data(), d, n * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n; ++i) out[i] = __half2float(h[i]);
+  return 0;
+}
+// B dense [H][W][C] images -> the RAFT shared-border layout: pixel (y, x) of image b at row b * raft_img_rows + y (W + pad) + x;
+// pad columns, pad rows and the tail rows of every image hold `fill`
+template <typename T, typename Cvt>
+std::vector<T> to_shared_border(const float* src, int B, int H, int W, int C, int pad, T fill, Cvt cvt) {
+  const long long ir = raft_img_rows(H, W, pad);
+  std::vector<T> m((size_t)B * ir * C, fill);
+  for (int b = 0; b < B; ++b)
+    for (int y = 0; y < H; ++y)
+      for (int x = 0; x < W; ++x)
+        for (int c = 0; c < C; ++c)
+          m[((size_t)b * ir + (size_t)y * (W + pad) + x) * C + c] = cvt(src[(((size_t)b * H + y) * W + x) * C + c]);
+  return m;
+}
 }  // namespace
 
 extern "C" {
@@ -701,6 +720,250 @@ int prisma_debug_da_preprocess(int device, const uint8_t* rgb, int h, int w, flo
   PRISMA_CUDA_OK(cudaMemcpy(di, rgb, (size_t)h * w * 3, cudaMemcpyHostToDevice));
   PRISMA_TRY(da_preprocess(di, h, w, dout, hn, wn, 0));
   PRISMA_CUDA_OK(cudaMemcpy(out, dout, (size_t)3 * hn * wn * 4, cudaMemcpyDeviceToHost));
+  return 0;
+  API_GUARD_END
+}
+
+// Kernel-level entries of the RAFT band's pointwise and gather kernels (raft_kernels.cu), with the conventions of the ViT
+// entries above.  Maps are built in the engine's shared-border layout (raft_img_rows): pad 1 for the encoder's maps, pad 2 for
+// the update block's, zero pad columns, pad rows and tail rows.
+int prisma_debug_raft_stem_im2col(int device, const float* x, int B, int H, int W, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(x != nullptr, "prisma_debug_raft_stem_im2col", "x", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_raft_stem_im2col", "out", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 64, "prisma_debug_raft_stem_im2col", "B", "must be in [1, 64]");
+  DEBUG_ARG(H >= 2 && H <= 4096 && H % 2 == 0, "prisma_debug_raft_stem_im2col", "H", "must be even, in [2, 4096]");
+  DEBUG_ARG(W >= 2 && W <= 4096 && W % 2 == 0, "prisma_debug_raft_stem_im2col", "W", "must be even, in [2, 4096]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_in = (size_t)B * 3 * H * W, n_out = (size_t)B * (H / 2) * (W / 2) * 192;
+  Scratch sc;
+  float* dx = sc.alloc<float>(n_in);
+  __half* dout = sc.alloc<__half>(n_out);
+  PRISMA_CHECK(dx && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dx, x, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 2));
+  PRISMA_TRY(raft_im2col_stem(dx, B, H, W, dout, 0));
+  return f16_to_host(dout, n_out, out);
+  API_GUARD_END
+}
+
+int prisma_debug_instnorm_stats(int device, const float* x, int B, int HW, int C, float* stats) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(x != nullptr, "prisma_debug_instnorm_stats", "x", "NULL");
+  DEBUG_ARG(stats != nullptr, "prisma_debug_instnorm_stats", "stats", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 64, "prisma_debug_instnorm_stats", "B", "must be in [1, 64]");
+  DEBUG_ARG(HW >= 1 && HW <= (1 << 24), "prisma_debug_instnorm_stats", "HW", "must be in [1, 2^24]");
+  DEBUG_ARG(C >= 1 && C <= 512, "prisma_debug_instnorm_stats", "C", "must be in [1, 512]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_in = (size_t)B * HW * C, n_st = (size_t)B * C * 2;
+  Scratch sc;
+  float* dx = sc.alloc<float>(n_in);
+  float* dpart = sc.alloc<float>(instnorm_partial_floats(B, HW, C));
+  float* dst = sc.alloc<float>(n_st);
+  PRISMA_CHECK(dx && dpart && dst, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dx, x, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dst, 0xFF, n_st * 4));
+  PRISMA_TRY(instnorm_stats(dx, B, HW, C, dpart, dst, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(stats, dst, n_st * 4, cudaMemcpyDeviceToHost));
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_instnorm_slab_stats(int device, const float* part, int B, int spi, int C, int HW, float* stats) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(part != nullptr, "prisma_debug_instnorm_slab_stats", "part", "NULL");
+  DEBUG_ARG(stats != nullptr, "prisma_debug_instnorm_slab_stats", "stats", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 64, "prisma_debug_instnorm_slab_stats", "B", "must be in [1, 64]");
+  DEBUG_ARG(spi >= 1 && spi <= (1 << 20), "prisma_debug_instnorm_slab_stats", "spi", "must be in [1, 2^20]");
+  DEBUG_ARG(C >= 1 && C <= 128, "prisma_debug_instnorm_slab_stats", "C", "must be in [1, 128]");
+  DEBUG_ARG(HW >= 1, "prisma_debug_instnorm_slab_stats", "HW", "must be >= 1");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_in = (size_t)B * spi * 2 * C, n_st = (size_t)B * C * 2;
+  Scratch sc;
+  float* dp = sc.alloc<float>(n_in);
+  double* dp2 = sc.alloc<double>((size_t)B * INSTNORM_STAGE1_BLOCKS * C * 2);
+  float* dst = sc.alloc<float>(n_st);
+  PRISMA_CHECK(dp && dp2 && dst, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dp, part, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dst, 0xFF, n_st * 4));
+  PRISMA_TRY(instnorm_stats_from_slabs(dp, B, spi, C, HW, dp2, dst, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(stats, dst, n_st * 4, cudaMemcpyDeviceToHost));
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_instnorm_apply(int device, const float* x, const float* stats, int B, int H, int W, int C, int skip_kind,
+                                const float* skip, const float* skip_stats, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(x != nullptr, "prisma_debug_instnorm_apply", "x", "NULL");
+  DEBUG_ARG(stats != nullptr, "prisma_debug_instnorm_apply", "stats", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_instnorm_apply", "out", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 64, "prisma_debug_instnorm_apply", "B", "must be in [1, 64]");
+  DEBUG_ARG(H >= 1 && H <= 4096, "prisma_debug_instnorm_apply", "H", "must be in [1, 4096]");
+  DEBUG_ARG(W >= 1 && W <= 4096, "prisma_debug_instnorm_apply", "W", "must be in [1, 4096]");
+  DEBUG_ARG(C >= 4 && C % 4 == 0 && C <= 512, "prisma_debug_instnorm_apply", "C", "must be a multiple of 4 in [4, 512]");
+  DEBUG_ARG(skip_kind >= 0 && skip_kind <= 2, "prisma_debug_instnorm_apply", "skip_kind", "must be 0 (none), 1 (fp16 map) or 2 (raw fp32)");
+  DEBUG_ARG(skip_kind == 0 || skip != nullptr, "prisma_debug_instnorm_apply", "skip", "NULL with skip_kind 1 or 2");
+  DEBUG_ARG(skip_kind != 2 || skip_stats != nullptr, "prisma_debug_instnorm_apply", "skip_stats", "NULL with skip_kind 2");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const long long ir = raft_img_rows(H, W, 1);
+  const size_t n_in = (size_t)B * H * W * C, n_st = (size_t)B * C * 2, n_out = (size_t)B * ir * C;
+  Scratch sc;
+  float* dx = sc.alloc<float>(n_in);
+  float* dst = sc.alloc<float>(n_st);
+  __half* dout = sc.alloc<__half>(n_out);
+  PRISMA_CHECK(dx && dst && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dx, x, n_in * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dst, stats, n_st * 4, cudaMemcpyHostToDevice));
+  __half* dskip_map = nullptr;
+  float *dskip_raw = nullptr, *dskip_st = nullptr;
+  if (skip_kind == 1) {  // the fp16 pad-1 map of the previous block's output
+    const std::vector<__half> h = to_shared_border(skip, B, H, W, C, 1, __float2half_rn(0.f), [](float v) { return __float2half_rn(v); });
+    dskip_map = sc.alloc<__half>(n_out);
+    PRISMA_CHECK(dskip_map, "cudaMalloc failed");
+    PRISMA_CUDA_OK(cudaMemcpy(dskip_map, h.data(), n_out * 2, cudaMemcpyHostToDevice));
+  } else if (skip_kind == 2) {  // the dense fp32 downsample conv output and its statistics
+    dskip_raw = sc.alloc<float>(n_in);
+    dskip_st = sc.alloc<float>(n_st);
+    PRISMA_CHECK(dskip_raw && dskip_st, "cudaMalloc failed");
+    PRISMA_CUDA_OK(cudaMemcpy(dskip_raw, skip, n_in * 4, cudaMemcpyHostToDevice));
+    PRISMA_CUDA_OK(cudaMemcpy(dskip_st, skip_stats, n_st * 4, cudaMemcpyHostToDevice));
+  }
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 2));
+  PRISMA_TRY(instnorm_apply(dx, dst, B, H, W, C, dskip_map, dskip_raw, dskip_st, dout, 1, ir, 0));
+  return f16_to_host(dout, n_out, out);
+  API_GUARD_END
+}
+
+int prisma_debug_raft_gru_operands(int device, const float* cn, int F, int B, int H, int W, const int* dir_frames,
+                                   const float* c0, const float* c1, float* h_master, float* hx, float* rhx) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(cn != nullptr, "prisma_debug_raft_gru_operands", "cn", "NULL");
+  DEBUG_ARG(dir_frames != nullptr, "prisma_debug_raft_gru_operands", "dir_frames", "NULL");
+  DEBUG_ARG(c0 != nullptr, "prisma_debug_raft_gru_operands", "c0", "NULL");
+  DEBUG_ARG(c1 != nullptr, "prisma_debug_raft_gru_operands", "c1", "NULL");
+  DEBUG_ARG(h_master != nullptr, "prisma_debug_raft_gru_operands", "h_master", "NULL");
+  DEBUG_ARG(hx != nullptr, "prisma_debug_raft_gru_operands", "hx", "NULL");
+  DEBUG_ARG(rhx != nullptr, "prisma_debug_raft_gru_operands", "rhx", "NULL");
+  DEBUG_ARG(F >= 1 && F <= 64, "prisma_debug_raft_gru_operands", "F", "must be in [1, 64]");
+  DEBUG_ARG(B >= 1 && B <= 8, "prisma_debug_raft_gru_operands", "B", "must be in [1, 8]");
+  DEBUG_ARG(H >= 1 && H <= 1024, "prisma_debug_raft_gru_operands", "H", "must be in [1, 1024]");
+  DEBUG_ARG(W >= 1 && W <= 1024, "prisma_debug_raft_gru_operands", "W", "must be in [1, 1024]");
+  DirFrames df;
+  for (int d = 0; d < 8; ++d) {
+    if (d < B) DEBUG_ARG(dir_frames[d] >= 0 && dir_frames[d] < F, "prisma_debug_raft_gru_operands", "dir_frames", "every entry must be in [0, F)");
+    df.f[d] = d < B ? dir_frames[d] : 0;
+  }
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const long long ir = raft_img_rows(H, W, 2);
+  const size_t n_cn = (size_t)F * H * W * 256, n_c = (size_t)B * 2 * H * W, rows = (size_t)B * ir;
+  Scratch sc;
+  float* dcn = sc.alloc<float>(n_cn);
+  float* dc0 = sc.alloc<float>(n_c);
+  float* dc1 = sc.alloc<float>(n_c);
+  float* dhm = sc.alloc<float>(rows * 128);
+  __half* dhx = sc.alloc<__half>(rows * 384);
+  __half* drhx = sc.alloc<__half>(rows * 384);
+  PRISMA_CHECK(dcn && dc0 && dc1 && dhm && dhx && drhx, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dcn, cn, n_cn * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dc0, c0, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dc1, c1, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dhm, 0xFF, rows * 128 * 4));
+  PRISMA_CUDA_OK(cudaMemset(dhx, 0xFF, rows * 384 * 2));
+  PRISMA_CUDA_OK(cudaMemset(drhx, 0xFF, rows * 384 * 2));
+  PRISMA_TRY(raft_cnet_split(dcn, B, H, W, 2, ir, df, dhm, dhx, drhx, 0));
+  PRISMA_TRY(raft_flow_cols(dc0, dc1, B, H, W, 2, ir, dhx, drhx, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(h_master, dhm, rows * 128 * 4, cudaMemcpyDeviceToHost));
+  PRISMA_TRY(f16_to_host(dhx, rows * 384, hx));
+  return f16_to_host(drhx, rows * 384, rhx);
+  API_GUARD_END
+}
+
+int prisma_debug_raft_flow_im2col(int device, const float* c0, const float* c1, int B, int H, int W, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(c0 != nullptr, "prisma_debug_raft_flow_im2col", "c0", "NULL");
+  DEBUG_ARG(c1 != nullptr, "prisma_debug_raft_flow_im2col", "c1", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_raft_flow_im2col", "out", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 8, "prisma_debug_raft_flow_im2col", "B", "must be in [1, 8]");
+  DEBUG_ARG(H >= 1 && H <= 1024, "prisma_debug_raft_flow_im2col", "H", "must be in [1, 1024]");
+  DEBUG_ARG(W >= 1 && W <= 1024, "prisma_debug_raft_flow_im2col", "W", "must be in [1, 1024]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const size_t n_c = (size_t)B * 2 * H * W, n_out = (size_t)B * H * W * 256;
+  Scratch sc;
+  float* dc0 = sc.alloc<float>(n_c);
+  float* dc1 = sc.alloc<float>(n_c);
+  __half* dout = sc.alloc<__half>(n_out);
+  PRISMA_CHECK(dc0 && dc1 && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dc0, c0, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dc1, c1, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 2));
+  PRISMA_TRY(raft_flow_im2col(dc0, dc1, B, H, W, dout, 0));
+  return f16_to_host(dout, n_out, out);
+  API_GUARD_END
+}
+
+int prisma_debug_raft_flow_head2(int device, const float* u, int B, int H, int W, float b0, float b1, const float* coords1_in,
+                                 float* coords1_out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(u != nullptr, "prisma_debug_raft_flow_head2", "u", "NULL");
+  DEBUG_ARG(coords1_in != nullptr, "prisma_debug_raft_flow_head2", "coords1_in", "NULL");
+  DEBUG_ARG(coords1_out != nullptr, "prisma_debug_raft_flow_head2", "coords1_out", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 8, "prisma_debug_raft_flow_head2", "B", "must be in [1, 8]");
+  DEBUG_ARG(H >= 1 && H <= 1024, "prisma_debug_raft_flow_head2", "H", "must be in [1, 1024]");
+  DEBUG_ARG(W >= 1 && W <= 1024, "prisma_debug_raft_flow_head2", "W", "must be in [1, 1024]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  // u as the 1x1 GEMM leaves it in the pad-2 map rows: zero pad columns, pad rows and tail rows
+  const std::vector<float> hu = to_shared_border(u, B, H, W, 32, 2, 0.f, [](float v) { return v; });
+  const size_t n_c = (size_t)B * 2 * H * W;
+  Scratch sc;
+  float* du = sc.alloc<float>(hu.size());
+  float* dc = sc.alloc<float>(n_c);
+  PRISMA_CHECK(du && dc, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(du, hu.data(), hu.size() * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dc, coords1_in, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_TRY(raft_flow_head2_gather(du, B, H, W, 2, raft_img_rows(H, W, 2), b0, b1, dc, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(coords1_out, dc, n_c * 4, cudaMemcpyDeviceToHost));
+  return 0;
+  API_GUARD_END
+}
+
+int prisma_debug_raft_convex_upsample(int device, const float* mask, const float* c0, const float* c1, int B, int H, int W,
+                                      int Hs, int Ws, int pad_top, int pad_left, float* out) {
+  API_GUARD_BEGIN
+  DEBUG_ARG(mask != nullptr, "prisma_debug_raft_convex_upsample", "mask", "NULL");
+  DEBUG_ARG(c0 != nullptr, "prisma_debug_raft_convex_upsample", "c0", "NULL");
+  DEBUG_ARG(c1 != nullptr, "prisma_debug_raft_convex_upsample", "c1", "NULL");
+  DEBUG_ARG(out != nullptr, "prisma_debug_raft_convex_upsample", "out", "NULL");
+  DEBUG_ARG(B >= 1 && B <= 8, "prisma_debug_raft_convex_upsample", "B", "must be in [1, 8]");
+  DEBUG_ARG(H >= 1 && H <= 1024, "prisma_debug_raft_convex_upsample", "H", "must be in [1, 1024]");
+  DEBUG_ARG(W >= 1 && W <= 1024, "prisma_debug_raft_convex_upsample", "W", "must be in [1, 1024]");
+  DEBUG_ARG(pad_top >= 0 && pad_top <= 7, "prisma_debug_raft_convex_upsample", "pad_top", "must be in [0, 7]");
+  DEBUG_ARG(pad_left >= 0 && pad_left <= 7, "prisma_debug_raft_convex_upsample", "pad_left", "must be in [0, 7]");
+  DEBUG_ARG(Hs >= 1 && Hs <= 8 * H - pad_top, "prisma_debug_raft_convex_upsample", "Hs", "must be in [1, 8 H - pad_top]");
+  DEBUG_ARG(Ws >= 1 && Ws <= 8 * W - pad_left, "prisma_debug_raft_convex_upsample", "Ws", "must be in [1, 8 W - pad_left]");
+  int sms = 0;
+  PRISMA_TRY(device_sms(device, &sms));
+  const std::vector<float> hm = to_shared_border(mask, B, H, W, 576, 2, 0.f, [](float v) { return v; });
+  const size_t n_c = (size_t)B * 2 * H * W, n_out = (size_t)B * Hs * Ws * 2;
+  Scratch sc;
+  float* dm = sc.alloc<float>(hm.size());
+  float* dc0 = sc.alloc<float>(n_c);
+  float* dc1 = sc.alloc<float>(n_c);
+  float* dout = sc.alloc<float>(n_out);
+  PRISMA_CHECK(dm && dc0 && dc1 && dout, "cudaMalloc failed");
+  PRISMA_CUDA_OK(cudaMemcpy(dm, hm.data(), hm.size() * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dc0, c0, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemcpy(dc1, c1, n_c * 4, cudaMemcpyHostToDevice));
+  PRISMA_CUDA_OK(cudaMemset(dout, 0xFF, n_out * 4));
+  PRISMA_TRY(raft_convex_upsample(dm, dc0, dc1, B, H, W, 2, raft_img_rows(H, W, 2), Hs, Ws, pad_top, pad_left, dout, 0));
+  PRISMA_CUDA_OK(cudaMemcpy(out, dout, n_out * 4, cudaMemcpyDeviceToHost));
   return 0;
   API_GUARD_END
 }

@@ -23,7 +23,7 @@ struct RMap {  // B NHWC fp16 maps in the shared-border layout: `pad` zero colum
   int B = 0, H = 0, W = 0, C = 0, pad = 1;
   int Hp() const { return H + pad; }
   int Wp() const { return W + pad; }
-  long long img_rows() const { return ((long long)Hp() * Wp() + 31) / 32 * 32; }  // a 32-row epilogue slab never straddles two images
+  long long img_rows() const { return raft_img_rows(H, W, pad); }
   long long rows() const { return B * img_rows(); }
 };
 
@@ -425,7 +425,7 @@ int RaftEngine::build_plan(int H, int W, double scale, int iters_) {
   PRISMA_TRY(r_alloc(plan_allocs, &stats_b, NF * 256 * 2));
   PRISMA_TRY(r_alloc(plan_allocs, &in_part, (size_t)instnorm_partial_floats(NF, (Hp_ / 2) * (Wp_ / 2), 128)));
   {  // per-slab (32 rows) column sums of the conv epilogues: the largest conv input is a pad-1 half-resolution map
-    const long long ir = (((long long)(Hp_ / 2 + 1) * (Wp_ / 2 + 1) + 31) / 32) * 32;
+    const long long ir = raft_img_rows(Hp_ / 2, Wp_ / 2, 1);
     slab_part_floats = (size_t)(round_up((int)(NF * ir), 256) / 32) * 2 * 128;  // CTA-pair tiles cover 256 rows
     PRISMA_TRY(r_alloc(plan_allocs, &slab_part, slab_part_floats));
     PRISMA_TRY(r_alloc(plan_allocs, &slab_part2, (size_t)NF * INSTNORM_STAGE1_BLOCKS * 128 * 2));

@@ -1,5 +1,5 @@
 // prisma_b200 -- RAFT band: the pointwise / gather kernels around the wgmma conv core
-// (instance norm, im2col of the 7x7 stem, cnet split, coords update, convex up-sampling).
+// (instance norm, im2col of the 7x7 stem, cnet split, flow im2col, FlowHead gather, convex up-sampling).
 // Reference: bands/raft/{extractor,update,raft}.py.  All feature maps are NHWC fp16 in the "shared border" layout: `pad`
 // zero columns after every row and `pad` zero rows after every image (gemm_tc.cuh GemmEpilogue::lead), so pixel (y, x) of
 // image b sits at row (b (H + pad) + y)(W + pad) + x.
@@ -305,24 +305,6 @@ __global__ void k_flow_cols(const float* __restrict__ c0, const float* __restric
 int raft_flow_cols(const float* c0, const float* c1, int B, int H, int W, int pad, long long img_rows, __half* hx, __half* rhx,
                    cudaStream_t s) {
   k_flow_cols<<<(unsigned)(((long long)B * H * W + 255) / 256), 256, 0, s>>>(c0, c1, B, H, W, pad, img_rows, hx, rhx);
-  PRISMA_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-// coords1 += delta_flow (raft.py:133); delta: fp32 padded rows [rows][4] (cols 0,1 used)
-__global__ void k_coords_update(const float* __restrict__ delta, int B, int H, int W, int pad, long long img_rows,
-                                float* __restrict__ coords1) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const int P = H * W;
-  if (idx >= (long long)B * P) return;
-  const int b = (int)(idx / P), r = (int)(idx - (long long)b * P);
-  const int y = r / W, x = r - y * W;
-  const int Wp = W + pad;  // shared-border layout: zeros only after each row / image
-  const size_t prow = (size_t)b * img_rows + (size_t)y * Wp + x;
-  coords1[(size_t)b * 2 * P + r] += delta[prow * 4];
-  coords1[(size_t)b * 2 * P + P + r] += delta[prow * 4 + 1];
-}
-int raft_coords_update(const float* delta, int B, int H, int W, int pad, long long img_rows, float* coords1, cudaStream_t s) {
-  k_coords_update<<<(unsigned)(((long long)B * H * W + 255) / 256), 256, 0, s>>>(delta, B, H, W, pad, img_rows, coords1);
   PRISMA_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -4,6 +4,10 @@
 
 namespace prisma {
 
+// Rows of one image in the shared-border layout of the RAFT maps: `pad` zero columns after every row and `pad` zero rows after
+// every image, rounded up to a multiple of 32 so that a 32-row epilogue slab never straddles two images.
+inline long long raft_img_rows(int H, int W, int pad) { return ((long long)(H + pad) * (W + pad) + 31) / 32 * 32; }
+
 int raft_im2col_stem(const float* x, int B, int H, int W, __half* out, cudaStream_t s);
 int instnorm_stats(const float* x, int B, int HW, int C, float* part, float* stats, cudaStream_t s);
 int instnorm_partial_floats(int B, int HW, int C);
@@ -19,7 +23,6 @@ int raft_cnet_split(const float* cn, int B, int H, int W, int pad, long long img
 int raft_flow_im2col(const float* c0, const float* c1, int B, int H, int W, __half* out, cudaStream_t s);
 int raft_flow_cols(const float* c0, const float* c1, int B, int H, int W, int pad, long long img_rows, __half* hx, __half* rhx,
                    cudaStream_t s);
-int raft_coords_update(const float* delta, int B, int H, int W, int pad, long long img_rows, float* coords1, cudaStream_t s);
 // FlowHead.conv2 as 1x1 GEMM partial products u [rows][32] (column tap*2 + out) + this nine-tap gather; coords1 += delta
 int raft_flow_head2_gather(const float* u, int B, int H, int W, int pad, long long img_rows, float b0, float b1, float* coords1,
                            cudaStream_t s);

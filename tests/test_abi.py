@@ -134,3 +134,67 @@ def test_debug_entries_refuse_bad_arguments_before_the_device(built_lib):
     assert "bad argument `heads`" in l.prisma_last_error().decode()
     assert l.prisma_debug_layernorm(0, p, p, p, p, 7, 500) < 0
     assert "bad argument `D`" in l.prisma_last_error().decode()
+
+
+def test_raft_debug_entries_refuse_bad_arguments_before_the_device(built_lib):
+    """The kernel-level entries of the RAFT band's pointwise and gather kernels check every argument before they touch the
+    device: each bad argument returns < 0 and prisma_last_error() names it, with or without a GPU (no launch is made here)."""
+    import ctypes as C
+    from prisma_b200._lib import fptr, lib
+    l = lib()
+    a = np.zeros(64, np.float32)
+    p, null = fptr(a), None
+    frames = (C.c_int * 8)(0, 1, 1, 2, 2, 3, 3, 4)
+    bad_frames = (C.c_int * 8)(0, 1, 1, 2, 2, 3, 3, 5)
+    cases = {
+        "prisma_debug_raft_stem_im2col": (
+            lambda x, B, H, W, o: l.prisma_debug_raft_stem_im2col(0, x, B, H, W, o),
+            dict(x=p, B=2, H=16, W=24, o=p),
+            [("x", dict(x=null)), ("out", dict(o=null)), ("B", dict(B=0)), ("H", dict(H=0)), ("H", dict(H=15)),
+             ("W", dict(W=-2)), ("W", dict(W=9))]),
+        "prisma_debug_instnorm_stats": (
+            lambda x, B, HW, Cc, s: l.prisma_debug_instnorm_stats(0, x, B, HW, Cc, s),
+            dict(x=p, B=2, HW=513, Cc=64, s=p),
+            [("x", dict(x=null)), ("stats", dict(s=null)), ("B", dict(B=0)), ("HW", dict(HW=0)), ("C", dict(Cc=0)),
+             ("C", dict(Cc=513))]),
+        "prisma_debug_instnorm_slab_stats": (
+            lambda pt, B, spi, Cc, HW, s: l.prisma_debug_instnorm_slab_stats(0, pt, B, spi, Cc, HW, s),
+            dict(pt=p, B=2, spi=40, Cc=96, HW=1000, s=p),
+            [("part", dict(pt=null)), ("stats", dict(s=null)), ("B", dict(B=0)), ("spi", dict(spi=0)), ("C", dict(Cc=0)),
+             ("C", dict(Cc=256)), ("HW", dict(HW=0))]),
+        "prisma_debug_instnorm_apply": (
+            lambda x, st, B, H, W, Cc, kind, sk, sks, o: l.prisma_debug_instnorm_apply(0, x, st, B, H, W, Cc, kind, sk, sks, o),
+            dict(x=p, st=p, B=2, H=5, W=7, Cc=64, kind=2, sk=p, sks=p, o=p),
+            [("x", dict(x=null)), ("stats", dict(st=null)), ("out", dict(o=null)), ("B", dict(B=0)), ("H", dict(H=0)),
+             ("W", dict(W=0)), ("C", dict(Cc=66)), ("C", dict(Cc=0)), ("skip_kind", dict(kind=3)), ("skip_kind", dict(kind=-1)),
+             ("skip", dict(kind=1, sk=null)), ("skip", dict(sk=null)), ("skip_stats", dict(sks=null))]),
+        "prisma_debug_raft_gru_operands": (
+            lambda cn, F, B, H, W, df, c0, c1, hm, hx, rhx: l.prisma_debug_raft_gru_operands(0, cn, F, B, H, W, df, c0, c1, hm, hx, rhx),
+            dict(cn=p, F=5, B=8, H=3, W=4, df=frames, c0=p, c1=p, hm=p, hx=p, rhx=p),
+            [("cn", dict(cn=null)), ("dir_frames", dict(df=null)), ("c0", dict(c0=null)), ("c1", dict(c1=null)),
+             ("h_master", dict(hm=null)), ("hx", dict(hx=null)), ("rhx", dict(rhx=null)), ("F", dict(F=0)), ("B", dict(B=9)),
+             ("B", dict(B=0)), ("H", dict(H=0)), ("W", dict(W=0)), ("dir_frames", dict(df=bad_frames)),
+             ("dir_frames", dict(F=4))]),
+        "prisma_debug_raft_flow_im2col": (
+            lambda c0, c1, B, H, W, o: l.prisma_debug_raft_flow_im2col(0, c0, c1, B, H, W, o),
+            dict(c0=p, c1=p, B=2, H=3, W=4, o=p),
+            [("c0", dict(c0=null)), ("c1", dict(c1=null)), ("out", dict(o=null)), ("B", dict(B=0)), ("B", dict(B=9)),
+             ("H", dict(H=0)), ("W", dict(W=0))]),
+        "prisma_debug_raft_flow_head2": (
+            lambda u, B, H, W, ci, co: l.prisma_debug_raft_flow_head2(0, u, B, H, W, 0.5, -0.25, ci, co),
+            dict(u=p, B=3, H=3, W=4, ci=p, co=p),
+            [("u", dict(u=null)), ("coords1_in", dict(ci=null)), ("coords1_out", dict(co=null)), ("B", dict(B=0)),
+             ("B", dict(B=9)), ("H", dict(H=0)), ("W", dict(W=0))]),
+        "prisma_debug_raft_convex_upsample": (
+            lambda m, c0, c1, B, H, W, Hs, Ws, pt, pl, o: l.prisma_debug_raft_convex_upsample(0, m, c0, c1, B, H, W, Hs, Ws, pt, pl, o),
+            dict(m=p, c0=p, c1=p, B=2, H=3, W=4, Hs=20, Ws=27, pt=3, pl=2, o=p),
+            [("mask", dict(m=null)), ("c0", dict(c0=null)), ("c1", dict(c1=null)), ("out", dict(o=null)), ("B", dict(B=0)),
+             ("H", dict(H=0)), ("W", dict(W=0)), ("pad_top", dict(pt=-1)), ("pad_top", dict(pt=8)), ("pad_left", dict(pl=8)),
+             ("Hs", dict(Hs=0)), ("Hs", dict(Hs=22)), ("Ws", dict(Ws=31)), ("Ws", dict(Ws=0))]),
+    }
+    for fn, (call, good, bad) in cases.items():
+        for arg, change in bad:
+            rc = call(**{**good, **change})
+            msg = l.prisma_last_error().decode()
+            assert rc < 0, (fn, arg, change)
+            assert f"{fn}: bad argument `{arg}`" in msg, (fn, arg, msg)
